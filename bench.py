@@ -76,7 +76,7 @@ def workload_config(map_points, scan_points, n_down):
     same seeded scans and the downsample being the same function — the same values.  Everything that describes how an arm
     runs it goes to `impl_config`."""
     return {"workload": WORKLOAD, "map_points": int(map_points), "scan_rays": 64 * N_AZ, "scan_points": float(scan_points),
-            "downsampled_points": float(n_down), "l2": "every step visits a different 120x80 m map block; table+points 4.3 GB >> 126 MB L2"}
+            "downsampled_points": float(n_down), "l2": "every step visits a different 120x80 m map block; table+points 4.3 GB >> 50 MB L2"}
 
 
 def step_block(s: int):
@@ -502,6 +502,8 @@ def main():
     ap.add_argument("--no-knn-batch", action="store_true")
     ap.add_argument("--no-shard-leg", action="store_true", help="N>1: skip the tile-sharded leg (replicas only)")
     ap.add_argument("--no-reference-order-leg", action="store_true", help="N=1: skip the extra leg with lsd_lio_set_reference_order off (sorted rows)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step returned "
+                    "(state vector, covariance, downsampled scan) as DIR/<name>.npy")
     ap.add_argument("--sweep-only", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--streams", type=int, default=4, help="extra leg (N=1): this many independent scan streams, each with "
                     "its own map replica and handle, registered concurrently on the one GPU (0/1 = skip)")
@@ -605,7 +607,7 @@ def main():
             if len(infos) >= 2:
                 infos[-2]["gpu_ms"] = info["gpu_ms"]  # async insert: device time is reported one scan late
         infos[-1]["gpu_ms"] = last_ms
-        return wall, infos, poses
+        return wall, infos, poses, (states[-1], covs[-1])
 
     def run_mode(sharded):
         """The value leg (scans resident in HBM) and the e2e leg (pinned host scans, H2D inside) of one multi-GPU mode."""
@@ -626,15 +628,16 @@ def main():
         sampler = ClockSampler(local)
         sampler.start()
         time.sleep(0.3)
-        wall_a, infos_a, poses_a = run_steps(lio, steps_a, dev_scans, W, prefetch=True)
+        wall_a, infos_a, poses_a, (state_a, cov_a) = run_steps(lio, steps_a, dev_scans, W, prefetch=True)
         clocks = sampler.stop()
+        outputs = {"state": state_a, "cov": cov_a, "downsampled_points": lio.get_down()}   # the last timed step's results
         xchg = lio.shard_exchange_stats() if sharded else None     # over the timed steps of the value leg
         host_scans = [torch.from_numpy(stp[0]).pin_memory() for stp in steps_b]
         scratch = torch.empty((131072, 4), dtype=torch.float32, device=dev)
         for hs in host_scans:  # first DMA from a freshly pinned buffer pays a one-off mapping cost: take it here
             scratch[:hs.shape[0]].copy_(hs, non_blocking=True)
         torch.cuda.synchronize()
-        wall_b, infos_b, _ = run_steps(lio, steps_b, host_scans, W, prefetch=not args.no_prefetch)
+        wall_b, infos_b, _, _ = run_steps(lio, steps_b, host_scans, W, prefetch=not args.no_prefetch)
         dev_ms = float(np.sum([i["gpu_ms"] for i in infos_a]))
         t = torch.tensor([wall_a, wall_b, dev_ms * 1e-3], dtype=torch.float64, device=dev)
         if dist is not None:
@@ -645,7 +648,7 @@ def main():
         streams = 1 if sharded else world
         return dict(xchg=xchg, lio=lio, st=st, build_s=build_s, steps_a=steps_a, steps_b=steps_b, dev_scans=dev_scans, host_scans=host_scans,
                     infos_a=infos_a, infos_b=infos_b, poses_a=poses_a, clocks=clocks, wall_a=wall_a, wall_b=wall_b, dev_s=dev_s,
-                    value=streams * K / wall_a, e2e=streams * K / wall_b, base=base)
+                    value=streams * K / wall_a, e2e=streams * K / wall_b, base=base, outputs=outputs)
 
     want_shard = world > 1 and args.mg_mode == "shard"
     main_run = run_mode(want_shard)
@@ -655,6 +658,11 @@ def main():
         other["lio"].close(); other["lio"] = None
     R = main_run
     lio, st, infos_a, infos_b = R["lio"], R["st"], R["infos_a"], R["infos_b"]
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in R["outputs"].items():
+            a = np.asarray(a)
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
     rho = st["points"] / max(st["cells"], 1)
 
     # H2D probe: what this box's PCIe path gives a 1.6 MB pinned copy (explains e2e - value)
@@ -699,7 +707,7 @@ def main():
         h.map.insert(m, 0)
         h.set_next_id(m.shape[0])
         h.set_reference_order(False)
-        wall_r, infos_r, poses_r = run_steps(h, R["steps_a"], R["dev_scans"], W, prefetch=True)
+        wall_r, infos_r, poses_r, _ = run_steps(h, R["steps_a"], R["dev_scans"], W, prefetch=True)
         ref_order_leg = {"value": K / wall_r, "unit": "scans/s", "ms_per_step": 1e3 * wall_r / K,
                          "device_ms_per_step": float(np.sum([i["gpu_ms"] for i in infos_r])) / K,
                          "vs_this_lines_value": (K / wall_r) / R["value"],
@@ -719,16 +727,10 @@ def main():
     alg_bytes = n_q * bytes_per_query
     dur_s = hs["ms"] / max(hs["count"], 1) * 1e-3
     achieved = alg_bytes / dur_s / 1e9 if dur_s > 0 else 0.0
-    peak, peak_src = 6650.0, "fallback"
+    peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3)"
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             peak, peak_src = float(json.load(f)["hbm_gbs"]), "measured"
-    except Exception:
-        pass
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            traffic = json.load(f).get("lio_hmodel_search_bytes_per_launch")
     except Exception:
         pass
 
@@ -821,7 +823,7 @@ def main():
         "gpu_launches": int(np.sum([i["kernel_launches"] for i in infos_a])),
         "pose_parity": pose_parity,
         "roofline": {"kernel": "lio_knn_kernel + lio_hmodel_kernel<search> (one search evaluation)", "bound": "hbm", "achieved": achieved, "peak": peak,
-                     "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+                     "peak_source": peak_src, "unit": "GB/s", "frac": achieved / peak,
                      "algorithmic_bytes_per_launch": alg_bytes, "bytes_per_query": bytes_per_query, "rho": rho,
                      "queries_per_launch": n_q, "us_per_launch": dur_s * 1e6, "launches_timed": hs["count"]},
         "kernels_ms": {k: (v["ms"] / max(v["count"], 1)) for k, v in prof.items()},

@@ -80,7 +80,7 @@ def ndt(args):
                alg_bytes_per_eval=float(scan.shape[0] * (16 + 7 * 16 + 3 * 52)),
                cost_gbs=float(scan.shape[0] * (16 + 7 * 16 + 3 * 52) / (cost_ms * 1e-3) / 1e9))
     if not args.no_ref_cuda and os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libref_cuda.so")):
-        # the reference's own CUDA NDT (NDTCudaCore + kernels, recompiled for sm_100a) on the same clouds, same GPU
+        # the reference's own CUDA NDT (NDTCudaCore + kernels, recompiled for sm_90a) on the same clouds, same GPU
         try:
             from oracle.reg import RefNdtCuda
             r = RefNdtCuda(0.5, 7)
@@ -89,11 +89,11 @@ def ndt(args):
             ra, Tr = t_ms(lambda: r.align(guess), 3)
             r.linearize(Tg)
             rl, _ = t_ms(lambda: r.linearize(Tg), 10)
-            out["reference_cuda_sm100a"] = dict(target_build_ms=rb, set_source_ms=rs, align_ms=ra, cost_eval_us=rl * 1e3, voxels=int(r.n_voxels),
+            out["reference_cuda_sm90a"] = dict(target_build_ms=rb, set_source_ms=rs, align_ms=ra, cost_eval_us=rl * 1e3, voxels=int(r.n_voxels),
                                                 converged=bool(r.converged), pos_err_m=float(np.abs(Tr[:3, 3] - tgt).max()))
             del r
         except Exception as e:  # the comparator must never take the measurement down
-            out["reference_cuda_sm100a"] = dict(error=repr(e)[:200])
+            out["reference_cuda_sm90a"] = dict(error=repr(e)[:200])
     if not args.no_cpu:
         near = (np.abs(m[:, 0] - tgt[0]) < 130) & (np.abs(m[:, 1] - tgt[1]) < 130)
         sub = np.ascontiguousarray(m[near])             # bounded CPU sample: the map within 130 m of the scan, full density
@@ -232,7 +232,7 @@ def gicp(args):
                    note="host clouds in, H2D + index build + covariances + align inside the timed region; rank r takes pairs r, r+N, ...")
         if (method == "FAST_VGICP" and world == 1 and not args.no_ref_cuda
                 and os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libref_cuda_vgicp.so"))):
-            # the reference's own CUDA VGICP (FastVGICPCuda + FastVGICPCudaCore, recompiled for sm_100a; "FAST_VGICP_CUDA",
+            # the reference's own CUDA VGICP (FastVGICPCuda + FastVGICPCudaCore, recompiled for sm_90a; "FAST_VGICP_CUDA",
             # registrations.cpp:43-55: neighbours from its CPU k-d tree, covariances / voxel map / LM loop on the GPU), same pair
             try:
                 from oracle.reg import RefVgicpCuda
@@ -241,12 +241,12 @@ def gicp(args):
                 rb, _ = t_ms(lambda: (r.set_target(m), r.set_source(src)))
                 r.align(guess)
                 ra, Tr = t_ms(lambda: r.align(guess), 3)
-                out["reference_cuda_sm100a"] = dict(method="FAST_VGICP_CUDA", covariance_build_ms=rb, align_ms=ra, converged=bool(r.converged),
+                out["reference_cuda_sm90a"] = dict(method="FAST_VGICP_CUDA", covariance_build_ms=rb, align_ms=ra, converged=bool(r.converged),
                                                     pos_err_m=float(np.abs(Tr[:3, 3] - tgt).max()),
                                                     note="first run on hardware pending (compiled after round 1's GPU budget was spent)")
                 del r
             except Exception as e:  # the comparator must never take the measurement down
-                out["reference_cuda_sm100a"] = dict(error=repr(e)[:200])
+                out["reference_cuda_sm90a"] = dict(error=repr(e)[:200])
         if not args.no_cpu and world == 1:
             m, src, guess, tgt = data[-1]
             from oracle import oracle as O

@@ -1,4 +1,4 @@
-/* lsdreg.h — C ABI of liblsdreg.so: the B200-native registration hot path for LSD.
+/* lsdreg.h — C ABI of liblsdreg.so: the H100-native registration hot path for LSD.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Every entry point is `extern "C"`, takes plain
  * pointers and sizes, returns an `lsd_status_t` (0 = ok, < 0 = error, > 0 = informational), never
@@ -14,7 +14,7 @@
  *     unless they must return a scalar; the plain variants take HOST pointers and include the
  *     H2D/D2H copies;
  *   - handles are confined to one thread at a time (SURVEY.md §8b "Thread-safety");
- *   - there is NO CPU fallback: every call fails with LSD_ERR_NO_DEVICE when no sm_100 GPU /
+ *   - there is NO CPU fallback: every call fails with LSD_ERR_NO_DEVICE when no sm_90 GPU /
  *     CUDA driver is present.
  */
 #ifndef LSDREG_H
@@ -223,7 +223,7 @@ lsd_status_t lsd_lio_reference_order_fallbacks(lsd_lio_t* l, unsigned* count);
  * 3 = serial replay (n > 32). */
 lsd_status_t lsd_debug_nth_element(const float* dist_host, int n, int first, int nth, int last, int* perm_out_host, int* path_out_host);
 /* Shape of the per-scan neighbour search (no reference counterpart): 0 or 1 = one warp per scan point (the only shape;
- * the flat shapes of round 1 measured slower on B200 and were retired). */
+ * the flat shapes of round 1 were retired). */
 lsd_status_t lsd_lio_set_knn_shape(lsd_lio_t* l, int shape);
 /* Programmatic dependent launch for the per-scan kernel chain (no reference counterpart; results are bit-identical either
  * way): flag != 0 launches the voxel-grid, search, h-model and map_incremental kernels with the programmatic stream

@@ -1,7 +1,7 @@
-"""lsdreg — B200-native registration hot path for LSD (lidar-slam-detection).
+"""lsdreg — H100-native registration hot path for LSD (lidar-slam-detection).
 
 Import as ``import lsdreg`` (alias module at the repo root; the directory name carries a hyphen).
-The compute path is liblsdreg.so (hand-written sm_100a CUDA behind a C ABI, include/lsdreg.h);
+The compute path is liblsdreg.so (hand-written sm_90a CUDA behind a C ABI, include/lsdreg.h);
 this package is its thin host-side mirror.  See DESIGN.md / INTEGRATION.md.
 """
 from . import shard, synth  # noqa: F401

@@ -209,7 +209,7 @@ SIGNATURES = [
 def load_library(path: str = LIB_PATH) -> C.CDLL:
     if not os.path.exists(path):
         raise ImportError(f"{path} not found: build it with `python __graft_entry__.py` "
-                          "(nvcc, sm_100a). lsdreg has no CPU fallback.")
+                          "(nvcc, sm_90a). lsdreg has no CPU fallback.")
     lib = C.CDLL(path)
     for name, res, args in SIGNATURES:
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol

@@ -1,8 +1,7 @@
 // brick.cuh — the brick layout of the hash-voxel map and the TMA-staged batched k-NN over it (K3, batch shape).
 //
-// Why: a hash of 128-byte voxel lines costs every query its own DRAM trips (tag -> line, per stencil cell) — measured in
-// round 1 at 1041 B of DRAM per query and 14 of 32 lanes active (profiles/r01k_knn_thread_ncu_raw.csv), 27-33 % of the HBM
-// roofline.  Here the same points are ALSO stored brick by brick: a brick is 8 x 8 x 4 voxels (4 x 4 x 2 m at 0.5 m) and its
+// Why: a hash of 128-byte voxel lines costs every query its own DRAM trips (tag -> line, per stencil cell), with most lanes
+// of a warp idle.  Here the same points are ALSO stored brick by brick: a brick is 8 x 8 x 4 voxels (4 x 4 x 2 m at 0.5 m) and its
 // page holds every point of those voxels PLUS a one-voxel halo (a point near a brick face is stored in up to 8 pages), so
 // the 19-cell NEARBY18 stencil of any query whose home voxel lies in the brick is answered from that ONE page.  A batch
 // is binned by brick (three small kernels), then a persistent CTA per work item pulls the page into shared memory with
@@ -41,9 +40,9 @@ static_assert(kPagePts % 16 == 0 && kPagePts + 16 * kBrickCap <= kPageBytes && k
 
 // A query in brick order, in one of two formats chosen per batch (brick_batch_is_ordered):
 //   32 bytes (x, y, z, w, index, pad) — one full sector per entry: a SHUFFLED batch scatters its entries all over the list, and a
-//     16-byte store into a sector somebody else completes later costs a read-modify-write (404 vs 438 us per 2 M queries);
+//     16-byte store into a sector somebody else completes later costs a read-modify-write;
 //   16 bytes (x, y, z, index) — a batch that arrives in spatial order fills both halves of a sector within one warp, and then
-//     half the bytes are simply half the bytes (351 vs 363 us: 61.6 % of the HBM roofline, profiles/r02y_*).
+//     half the bytes are simply half the bytes.
 struct __align__(32) BrickQuery { float4 p; int qi; int pad[3]; };
 __device__ __forceinline__ void brick_query_store(BrickQuery* list, int pos, float4 q, int i, bool compact) {
   if (compact) reinterpret_cast<float4*>(list)[pos] = make_float4(q.x, q.y, q.z, __int_as_float(i));
@@ -233,7 +232,7 @@ __global__ void __launch_bounds__(256) brick_bin_kernel(BrickView bv, float inv_
 // K-B: one thread per directory slot: a contiguous range of the sorted query list for every brick that has queries, cut
 // into work items of <= kBrickQC queries.  ctr[0] = queries placed, ctr[1] = work items.  Leaves bin_count zeroed.
 // The two running totals are claimed once per BLOCK (block-wide exclusive scan, then one atomicAdd each): one atomic per
-// occupied slot on the same two words serialised the whole kernel (232 us for 160 k bricks, profiles/r02b).
+// occupied slot on the same two words serialises the whole kernel.
 __device__ __forceinline__ unsigned block_excl_scan_256(unsigned v, unsigned* warp_tot, unsigned* total) {
   const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned inc = v;
@@ -289,8 +288,8 @@ __global__ void __launch_bounds__(256) brick_scatter_kernel(const float4* __rest
 // lane 0 claims the next item and issues the page's bulk copies, the lanes load their queries meanwhile, the warp waits
 // on the barrier and answers the item's queries from shared memory.
 //
-// What the instruction profile of the first two versions asked for (profiles/r02c, r02d: issue-bound at 85 % with 6-10 of
-// 32 lanes active, half of the instructions in a branchy insertion running 3-5 lanes wide):
+// What the instruction profile of the first two versions asked for (issue-bound with a minority of the 32 lanes active,
+// half of the instructions in a branchy insertion running a few lanes wide):
 //  * lane groups — a brick of the benchmark batch has ~13 queries, so an item of qn queries gives each query
 //    g = 32 / pow2ceil(qn) lanes (1, 2, 4 or 8); lane `sub` of a group takes stencil cells sub, sub + g, ...
 //  * a FLAT walk — phase 1 collects the heads of the lane's non-empty cells into a 28-byte queue in shared memory (uniform

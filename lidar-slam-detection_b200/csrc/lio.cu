@@ -27,7 +27,7 @@ namespace lsd {
 
 constexpr int kNV = 32;        // reduction slots per block (29 used + n)
 constexpr int kLioBlock = 256;
-constexpr int kLioMaxGrid = 296;  // 2 blocks per SM: the final fold reads <= 296 x 32 partials
+constexpr int kLioMaxGrid = 2 * kNumSms;  // 2 blocks per SM: the final fold reads <= kLioMaxGrid x 32 partials
 
 struct LioPose { double R[9], t[3], RL[9], tL[3]; };
 
@@ -339,12 +339,10 @@ __constant__ unsigned char c_tri[21][2] = {{0,0},{0,1},{0,2},{0,3},{0,4},{0,5},{
 // pinned id for id to the compiled iVox.  A query whose candidates overflow the search's list (kCandCap = 256) is answered in
 // the canonical (d2, id) order and counted (lsd_lio_reference_order_fallbacks).
 //
-// History of where the replay ran (B200, per search evaluation, 12 k queries): one thread per query on per-thread local arrays
-// inside the plane-fit kernel +65 us; on shared memory but inlined three times +135 us (it took that kernel's registers); its
-// own 64-thread-block kernel +31 us, with batched global loads +27 us — a chain of ~3 k dependent instructions per thread,
-// one warp per scheduler, nothing to hide latency behind; by the search's own warp, below, +11 us (DESIGN.md section 6).  Gathering
-// cell by cell (warp prefix sum of per-cell counts) so that the list is the sequence without the all-pairs placement was
-// tried last and cost 6 us MORE (seven distances and ids per lane held in registers): profiles/r02zc_*_not_kept.jsonl.
+// Where the replay runs: one thread per query inside the plane-fit kernel takes that kernel's registers, and a kernel of its
+// own is a chain of ~3 k dependent instructions per thread with nothing to hide latency behind; the search's own warp,
+// below, keeps the lanes busy.  Gathering cell by cell (warp prefix sum of per-cell counts) so that the list is the sequence
+// without the all-pairs placement needs seven distances and ids per lane held in registers.
 #ifdef LSD_SIMT_EMU
 #define RS_INL __device__
 #define RS_ONE __device__
@@ -1490,7 +1488,7 @@ lsd_status_t lsd_lio_create(lsd_lio_t** out, const lsd_lio_params_t* p) {
   if (s) { lsd_map_destroy(l->map); delete l; return s; }
   const size_t mp = (size_t)p->max_points;
   const size_t max_blocks = (size_t)grid_for(p->max_points) + 1;
-  l->max_search_blocks = 148 * 6;
+  l->max_search_blocks = lsd::kNumSms * 6;
   cudaError_t e = cudaStreamCreateWithFlags(&l->stream, cudaStreamNonBlocking);
   auto A = [&](void** ptr, size_t b) { if (e == cudaSuccess) e = cudaMalloc(ptr, b); if (e == cudaSuccess) e = cudaMemset(*ptr, 0, b); };
   for (int i = 0; i < 2; i++) {
@@ -1534,9 +1532,9 @@ lsd_status_t lsd_lio_create(lsd_lio_t** out, const lsd_lio_params_t* p) {
   cudaStreamDestroy(l->vg->stream); l->vg->stream = l->stream;
   // The voxel grid of an announced scan is pipelined under the running one by default (bit-identical results,
   // tests/test_gpu_zz_pdl.py; LSD_PIPELINE_VG=0 / lsd_lio_set_pipeline turn it off).  Programmatic dependent launch stays
-  // opt-in (LSD_PDL=1 / lsd_lio_set_pdl): measured on B200 in one process on one box (profiles/r02d_lio_probe.jsonl) it
-  // shortens the device time per scan but cudaLaunchKernelEx costs the host ~2.5 us more per launch than a plain triple-chevron launch, and with
-  // a host loop that is synchronous per evaluation that is on the critical path: 4779 scans/s with it, 5649 without.
+  // opt-in (LSD_PDL=1 / lsd_lio_set_pdl): it shortens the device time per scan, but cudaLaunchKernelEx costs the host more
+  // per launch than a plain triple-chevron launch, and with a host loop that is synchronous per evaluation that is on the
+  // critical path.
   { const char* ev = getenv("LSD_PDL"); l->pdl = (ev && ev[0] == '1') ? 1 : 0; }
   { const char* ev = getenv("LSD_PIPELINE_VG"); l->pipeline_vg = (ev && ev[0] == '0') ? 0 : 1; }
   // The reference's Nearest_Points rows outlive a search that finds nothing (laserMapping.cpp:1273, ivox3d.h:155-157);
@@ -1544,12 +1542,10 @@ lsd_status_t lsd_lio_create(lsd_lio_t** out, const lsd_lio_params_t* p) {
   l->stale_rows = true;
   // The neighbours reach esti_plane in the order IVox::GetClosestPoint returns them (DESIGN.md section 4: what takes the
   // posterior from ~4e-5 m to ~2e-7 m of laserMapping.cpp's); LSD_REF_ORDER=0 / lsd_lio_set_reference_order(l, 0) give the
-  // 9 % faster sorted order instead.
+  // faster sorted order instead.
   { const char* ev = getenv("LSD_REF_ORDER"); lsd_status_t r = lsd_lio_set_reference_order(l, (ev && ev[0] == '0') ? 0 : 1); if (r) { lsd_lio_destroy(l); return r; } }
-  {  // cluster-shaped reuse evaluation: opt-in, LSD_REUSE_CLUSTER="CxT" = C CTAs of T threads.  Measured slower than the
-     // grid-wide kernel in every shape tried on B200 (15.6 us vs 21.5 us for 16 x 256 ... 56 us for 2 x 1024,
-     // profiles/r02d_lio_probe.jsonl): the per-pass shuffle reduction that keeps it inside 64 registers costs more than the
-     // partials -> ticket -> last-block fold it replaces.
+  {  // cluster-shaped reuse evaluation: opt-in, LSD_REUSE_CLUSTER="CxT" = C CTAs of T threads.  The per-pass shuffle
+     // reduction that keeps it inside 64 registers can cost more than the partials -> ticket -> last-block fold it replaces.
     const char* ev = getenv("LSD_REUSE_CLUSTER");
     l->reuse_cluster = (ev && ev[0] >= '1' && ev[0] <= '9') ? 1 : 0;
     int c = 0, t = 0;

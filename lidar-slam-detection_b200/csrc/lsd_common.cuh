@@ -1,4 +1,4 @@
-// lsd_common.cuh — shared device/host helpers for liblsdreg (sm_100a only).
+// lsd_common.cuh — shared device/host helpers for liblsdreg (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -8,6 +8,9 @@
 #include "../../include/lsdreg.h"
 
 namespace lsd {
+
+// SMs of the H100 SXM: persistent and grid-stride launches are sized in multiples of it
+constexpr int kNumSms = 132;
 
 // ------------------------------------------------------------------ errors
 void set_error(const char* fmt, ...);

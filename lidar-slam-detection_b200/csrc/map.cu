@@ -5,7 +5,7 @@
 //                                                  atomicAdd slot claim, float4 stores)
 //   GetClosestPoint :139-171 -> knn_query_kernel   (knn.cuh)
 // The LRU list of the reference (ivox3d.h:246-255) is not reproduced: the table is sized for the
-// whole map in HBM (180 GB) instead of evicting at 100 000 voxels.
+// whole map in HBM (80 GB on an H100) instead of evicting at 100 000 voxels.
 #include <stdarg.h>
 #include <stdlib.h>
 
@@ -344,7 +344,7 @@ static lsd_status_t launch_knn_bricks(lsd_map* m, const float4* d_q, int nq, int
   brick_bin_kernel<<<gq, 256, 0, st>>>(bv, m->view.inv_res, d_q, nq, k, q_slot, q_rank, m->bin_count, d_idx, d_d2, d_cnt, ctr + 3);
   brick_plan_kernel<<<(unsigned)((m->n_bricks + 255) / 256), 256, 0, st>>>(bv, m->n_bricks, m->bin_count, m->bin_base, work, ctr);
   brick_scatter_kernel<<<gq, 256, 0, st>>>(d_q, q_slot, q_rank, m->bin_base, nq, sorted, ctr);
-  const int grid = (int)std::min<size_t>(148 * 5, (n_work_max + kBrickWarps - 1) / kBrickWarps);   // 5 CTAs x 4 warps x 2 x 4.6 KB per SM
+  const int grid = (int)std::min<size_t>(lsd::kNumSms * 5, (n_work_max + kBrickWarps - 1) / kBrickWarps);   // 5 CTAs x 4 warps x 2 x 4.6 KB per SM
   if (k == 1) brick_knn_kernel<1><<<grid, kBrickWarps * 32, 0, st>>>(bv, m->view.inv_res, st_slot, max_sq, sorted, nq, work, ctr, d_idx, d_d2, d_cnt);
   else brick_knn_kernel<5><<<grid, kBrickWarps * 32, 0, st>>>(bv, m->view.inv_res, st_slot, max_sq, sorted, nq, work, ctr, d_idx, d_d2, d_cnt);
   LSD_CUDA(cudaGetLastError());
@@ -510,7 +510,7 @@ lsd_status_t launch_knn(lsd_map* m, const float4* d_q, int nq, int k, float max_
     m->launches++;
     return LSD_OK;
   }
-  dim3 g(std::min((nq + kKnnWarps - 1) / kKnnWarps, 148 * 8)), b(kKnnWarps * 32);
+  dim3 g(std::min((nq + kKnnWarps - 1) / kKnnWarps, lsd::kNumSms * 8)), b(kKnnWarps * 32);
   switch (k) {
     case 1: knn_query_kernel<1><<<g, b, 0, st>>>(m->view, d_q, nq, max_sq, stencil, d_idx, d_d2, d_cnt); break;
     case 5: knn_query_kernel<5><<<g, b, 0, st>>>(m->view, d_q, nq, max_sq, stencil, d_idx, d_d2, d_cnt); break;
@@ -529,7 +529,7 @@ using namespace lsd;
 // ==================================================================== C ABI
 extern "C" {
 
-const char* lsd_version(void) { return "lsdreg 0.1.0 (sm_100a)"; }
+const char* lsd_version(void) { return "lsdreg 0.1.0 (sm_90a)"; }
 const char* lsd_last_error(void) { return g_err; }
 
 lsd_status_t lsd_init(int device) {
@@ -539,8 +539,8 @@ lsd_status_t lsd_init(int device) {
   if (device < 0 || device >= n) { set_error("device %d out of range (%d devices)", device, n); return LSD_ERR_INVALID; }
   g_device = device;
   LSD_CUDA(cudaSetDevice(device));
-  // L2 fetch granularity stays at the driver default: measured on B200 (profiles/r01_knn_batch.txt), asking
-  // for 32-byte fetches halves the DRAM bytes of a hash probe but makes the batched k-NN 19 % SLOWER.
+  // L2 fetch granularity stays at the driver default: 32-byte fetches halve the DRAM bytes of a hash probe but
+  // can make the batched k-NN slower.
   // LSD_L2_FETCH_GRANULARITY=32|64|128 overrides it for A/B measurements.
   if (const char* e = getenv("LSD_L2_FETCH_GRANULARITY")) {
     const size_t g = (size_t)atoi(e);

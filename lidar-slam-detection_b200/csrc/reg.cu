@@ -766,7 +766,7 @@ static lsd_status_t reg_wait(lsd_reg* r, double seq) {
 
 constexpr int kThreadShapeMin = 16384;  // clouds from this size on use the thread-per-point search kernels
 static int reg_grid(int n) { return std::max(1, std::min((n + 255) / 256, kLioMaxGrid)); }
-static int warp_grid(int n) { return std::max(1, std::min((n + kRegWarps - 1) / kRegWarps, 148 * 6)); }
+static int warp_grid(int n) { return std::max(1, std::min((n + kRegWarps - 1) / kRegWarps, lsd::kNumSms * 6)); }
 
 // linearize (update = true) / compute_error at T.  H36/b6 may be null.
 static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H36, double* b6, double* err, int* n_corr) {
@@ -1050,7 +1050,7 @@ lsd_status_t lsd_reg_create(lsd_reg_t** out, const lsd_reg_params_t* p) {
   r->sc.world = 1;
   for (int i = 0; i < 16; i++) r->final_T[i] = r->lin_T[i] = (i % 5 == 0) ? 1.0 : 0.0;
   cudaError_t e = cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&r->d_partials, (size_t)(148 * 6 + 8) * kNV * 8);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&r->d_partials, (size_t)(lsd::kNumSms * 6 + 8) * kNV * 8);
   if (e == cudaSuccess) e = cudaMalloc((void**)&r->d_done, 64);
   if (e == cudaSuccess) e = cudaMemset(r->d_done, 0, 64);
   if (e == cudaSuccess) e = cudaHostAlloc((void**)&r->h_result, kResDoubles * 8, cudaHostAllocMapped);

@@ -216,7 +216,7 @@ static lsd_status_t sc_make_dev(lsd_sc* s, const float4* d_pts, int n, const dou
   LSD_CUDA(cudaMemcpyAsync(s->d_off, offsets_xy, (size_t)n_off * 16, cudaMemcpyHostToDevice, st));
   sc_fill_kernel<<<(n_off * kDesc + 255) / 256, 256, 0, st>>>(s->d_enc, n_off * kDesc);
   if (n > 0) {
-    const int nb = std::max(1, std::min((n + kScBinBlock * 4 - 1) / (kScBinBlock * 4), 148));
+    const int nb = std::max(1, std::min((n + kScBinBlock * 4 - 1) / (kScBinBlock * 4), lsd::kNumSms));
     sc_bin_kernel<<<dim3(nb, n_off), kScBinBlock, 0, st>>>(d_pts, n, s->d_off, s->d_enc);
     s->launches++;
   }

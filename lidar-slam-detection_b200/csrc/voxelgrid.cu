@@ -341,9 +341,9 @@ __global__ void __launch_bounds__(256) vg_sum_kernel(const float4* __restrict__ 
 lsd_status_t vg_run(lsd_voxelgrid* g, const float4* d_in, int n, float leaf, float4* d_out, int* d_m, cudaStream_t st) {
   if (n > g->max_points) { set_error("voxelgrid: %d points exceed capacity %d", n, g->max_points); return LSD_ERR_CAPACITY; }
   if (n <= 0) { LSD_CUDA(cudaMemsetAsync(d_m, 0, sizeof(int), st)); return LSD_OK; }
-  const int nb = std::min((n + 255) / 256, 592);
+  const int nb = std::min((n + 255) / 256, 4 * lsd::kNumSms);
   const int pdl = g->pdl;
-  LSD_LAUNCH(pdl, vg_minmax_kernel, std::min(nb, 148), 256, st, d_in, n, g->bbox);
+  LSD_LAUNCH(pdl, vg_minmax_kernel, std::min(nb, lsd::kNumSms), 256, st, d_in, n, g->bbox);
   LSD_LAUNCH(pdl, vg_mark_kernel, nb, 256, st, d_in, n, leaf, g->max_cells, g->bbox, g->grid, g->bitmap, g->vidx);
   LSD_LAUNCH(pdl, vg_scan_kernel, g->scan_blocks, 256, st, g->grid, g->bitmap, g->word_prefix, g->chunk_sum, g->done, d_m, n);
   if (g->input_order_sums) {
@@ -380,8 +380,7 @@ lsd_status_t lsd_voxelgrid_create(lsd_voxelgrid_t** out, int max_points, int log
   g->max_cells = log2_max_cells == 31 ? 2147483647ll : (1ll << log2_max_cells);
   const size_t words = (size_t)((g->max_cells + 31) >> 5);
   const size_t chunks = (words + kScanChunk - 1) / kScanChunk;
-  g->scan_blocks = (int)std::min<size_t>(chunks, 1184);
-  g->scan_blocks = (int)std::min<size_t>(g->scan_blocks, 296);
+  g->scan_blocks = (int)std::min<size_t>(chunks, 2 * lsd::kNumSms);
   cudaError_t e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking);
   auto A = [&](void** p, size_t b) { if (e == cudaSuccess) e = cudaMalloc(p, b); if (e == cudaSuccess) e = cudaMemset(*p, 0, b); };
   A((void**)&g->bbox, 8 * sizeof(int));

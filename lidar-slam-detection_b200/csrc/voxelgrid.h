@@ -14,7 +14,7 @@ struct VgGrid {  // device-resident grid description, written by vg_setup_kernel
 }  // namespace lsd
 
 struct lsd_voxelgrid {
-  int device = 0, max_points = 0, scan_blocks = 0, coop_blocks = 148;
+  int device = 0, max_points = 0, scan_blocks = 0, coop_blocks = lsd::kNumSms;
   long long max_cells = 0;
   cudaStream_t stream = nullptr;
   int* bbox = nullptr;            // ordered-int min[3], max[3]

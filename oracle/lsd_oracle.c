@@ -792,7 +792,7 @@ int orc_map_incremental(OrcIvox* map, const float* body, int n, const double* R,
 /*        .../find_voxel_correspondences.cu:16-111, ndt_compute_derivatives.cu:15-102      */
 /*        include/fast_gicp/cuda/vector3_hash.cuh:35-38 (coord = floor(x/res - 0.5))       */
 /*      Pin status: the reference NDT exists only as CUDA (thrust) code; it recompiles for  */
-/*      sm_100a (oracle/ref_cuda.cu) and pins this restatement on the GPU box               */
+/*      sm_90a (oracle/ref_cuda.cu) and pins this restatement on the GPU box               */
 /*      (tests/test_gpu_ref_cuda.py), within the bounds its lossy voxel table allows.       */
 /*      fp32 per-element arithmetic as the reference; sums are carried in double (the      */
 /*      reference reduces fp32 tuples in thrust's unspecified tree order).                 */

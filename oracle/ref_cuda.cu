@@ -1,13 +1,13 @@
 // TEST INFRASTRUCTURE ONLY — never linked into the product (liblsdreg.so).
 //
 // C-ABI wrapper around the UNMODIFIED reference CUDA matcher, compiled where it lies under
-// /root/reference/slam/thirdparty/fast_gicp by oracle/Makefile (nvcc, sm_100a) into oracle/_ref/libref_cuda.so:
+// /root/reference/slam/thirdparty/fast_gicp by oracle/Makefile (nvcc, sm_90a) into oracle/_ref/libref_cuda.so:
 //   * fast_gicp::cuda::NDTCudaCore + its kernels   src/fast_gicp/cuda/{ndt_cuda,gaussian_voxelmap,
 //         find_voxel_correspondences,ndt_compute_derivatives,covariance_regularization}.cu
 //   * fast_gicp::NDTCuda (LsqRegistration LM loop)  include/fast_gicp/ndt/impl/ndt_cuda_impl.hpp,
 //                                                  include/fast_gicp/gicp/impl/lsq_registration_impl.hpp
 // It needs a GPU to run, so it is used by the `-m gpu` tests and by bench_extra.py's "reference kernels" leg:
-// the reference's own CUDA code, recompiled for sm_100a, on the same B200 as liblsdreg.
+// the reference's own CUDA code, recompiled for sm_90a, on the same H100 as liblsdreg.
 // PCL / Boost are shimmed exactly as for oracle/ref_reg.cpp (oracle/ref_shim_reg, ours).
 #include <pcl/point_types.h>
 #include <pcl/point_cloud.h>

@@ -3,7 +3,7 @@
 // C-ABI wrapper around the UNMODIFIED reference CUDA VGICP matcher — the method the reference selects by default where it
 // is built with USE_VGICP_CUDA (hdl_graph_slam/registrations.cpp:25-27,43-55; global_localization.cpp:18;
 // scan_matching_odometry_nodelet.cpp:122) — compiled where it lies under /root/reference/slam/thirdparty/fast_gicp by
-// oracle/Makefile (nvcc, sm_100a) into oracle/_ref/libref_cuda_vgicp.so:
+// oracle/Makefile (nvcc, sm_90a) into oracle/_ref/libref_cuda_vgicp.so:
 //   * fast_gicp::cuda::FastVGICPCudaCore + kernels   src/fast_gicp/cuda/{fast_vgicp_cuda,brute_force_knn,compute_derivatives,
 //         compute_mahalanobis,covariance_estimation,covariance_estimation_rbf,covariance_regularization,gaussian_voxelmap,
 //         find_voxel_correspondences}.cu

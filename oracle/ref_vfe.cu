@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY — never linked into the product (liblsdreg.so).
 //
 // C-ABI wrapper around the UNMODIFIED reference detection voxelizer, compiled where it lies under
-// /root/reference/sensor_driver/inference/voxelize by oracle/Makefile (nvcc, sm_100a) into oracle/_ref/libref_vfe.so:
+// /root/reference/sensor_driver/inference/voxelize by oracle/Makefile (nvcc, sm_90a) into oracle/_ref/libref_vfe.so:
 //   * Preprocess::forward     preprocess_kernel.cu:56-101   (sliding window, motion compensation)
 //   * Voxelization::forward   voxelization_kernel.cu:225-255 (hash voxelisation, mean, fp16)
 // Runs only where a GPU is present (the `-m gpu` tests); pins lsd_vfe_* against the reference's own kernels.

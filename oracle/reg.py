@@ -7,7 +7,7 @@
 Pin status: the GICP / VGICP cost functions, the covariances, se3_exp and the whole LM loop are checked
 against the COMPILED reference classes (oracle/ref_reg.cpp -> oracle/_ref/libref_reg.so: the reference's
 own LsqRegistration / FastGICP / FastVGICP headers, with our PCL/Boost shims) in tests/test_oracle_reg.py.
-NDT (P2D): the reference NDT exists only as CUDA code; its own sources recompile for sm_100a
+NDT (P2D): the reference NDT exists only as CUDA code; its own sources recompile for sm_90a
 (oracle/ref_cuda.cu -> oracle/_ref/libref_cuda.so, RefNdtCuda below) and pin the NDT restatement and the product's
 NDT kernels on the GPU box (tests/test_gpu_ref_cuda.py).
 """
@@ -271,7 +271,7 @@ def ref_se3_exp(a):
 
 
 class RefNdtCuda:
-    """The COMPILED reference CUDA NDT (fast_gicp::NDTCuda over NDTCudaCore), sm_100a build; needs a GPU."""
+    """The COMPILED reference CUDA NDT (fast_gicp::NDTCuda over NDTCudaCore), sm_90a build; needs a GPU."""
     _lib = None
 
     def __init__(self, resolution=1.0, neighbors=7, max_iterations=64, trans_eps=0.01, rot_eps=0.1):
@@ -313,7 +313,7 @@ class RefNdtCuda:
 
 
 class RefVgicpCuda:
-    """The COMPILED reference CUDA VGICP (fast_gicp::FastVGICPCuda over FastVGICPCudaCore), sm_100a build; needs a GPU.
+    """The COMPILED reference CUDA VGICP (fast_gicp::FastVGICPCuda over FastVGICPCudaCore), sm_90a build; needs a GPU.
     Parameters of registrations.cpp:43-55 ("FAST_VGICP_CUDA"): resolution 1.0, eps 0.01, 64 iterations, k = 20, source /
     target neighbours from a CPU k-d tree (nn_method 0), DIRECT1 voxel correspondences."""
     _lib = None

@@ -5,7 +5,7 @@ Follows sensor_driver/inference/voxelize (relative to /root/reference):
   voxelization_kernel.cu:73-180      hash voxelisation, <= max_points_per_voxel points, mean, fp16
 executed SEQUENTIALLY in point order (the reference's GPU result depends on thread arrival order;
 the sequential order is one of its possible outcomes).  Pin status: the reference has no CPU implementation of this
-path, but its two .cu files recompile unmodified for sm_100a (oracle/ref_vfe.cu -> oracle/_ref/libref_vfe.so, class
+path, but its two .cu files recompile unmodified for sm_90a (oracle/ref_vfe.cu -> oracle/_ref/libref_vfe.so, class
 RefVoxelizer below) and pin this restatement's semantics and the product on the GPU box (tests/test_gpu_ref_cuda.py).
 """
 from __future__ import annotations
@@ -91,7 +91,7 @@ class OracleVoxelizer:
 
 
 class RefVoxelizer:
-    """The COMPILED reference voxelizer (Preprocess + Voxelization kernels recompiled for sm_100a:
+    """The COMPILED reference voxelizer (Preprocess + Voxelization kernels recompiled for sm_90a:
     oracle/ref_vfe.cu -> oracle/_ref/libref_vfe.so).  Needs a GPU; loaded lazily."""
     _lib = None
 

@@ -9,13 +9,13 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 with -m gpu)")
     # make sure the native artefacts exist (nvcc cross-compiles without a GPU)
     import __graft_entry__ as g
     g.build()   # no-op when liblsdreg.so, slam_wrapper and the oracle libraries are newer than their sources
     if os.environ.get("LSDREG_EMU"):
         # run the `gpu` tests against the SIMT emulator build (tests/simt): the same sources, kernels executed by fibers on
-        # the CPU.  A debugging aid for kernels written without a GPU at hand; never a substitute for the B200 run.
+        # the CPU.  A debugging aid for kernels written without a GPU at hand; never a substitute for the H100 run.
         sys.path.insert(0, os.path.join(ROOT, "tests", "simt"))
         import build_emu
         import lsdreg

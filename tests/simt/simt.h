@@ -1,5 +1,5 @@
 // simt.h — TEST INFRASTRUCTURE.  A single-OS-thread SIMT emulator that runs the product's CUDA sources on the host, so
-// that kernels written while no GPU is available can be executed against the oracle before they ever see a B200
+// that kernels written while no GPU is available can be executed against the oracle before they ever see a GPU
 // (tests/simt/README.md).  It is NOT a CPU path of the product: liblsdreg.so never contains it; tests build a separate
 // liblsdreg_emu.so from translated copies of the sources (tests/simt/build_emu.py) and load it explicitly.
 //

@@ -2,15 +2,15 @@
 10.1 M-point map, full iterate-to-converge, every step in another block) through lsd_lio_scan, against
 
   (a) laserMapping.cpp COMPILED UNMODIFIED (oracle/_ref/libref_fastlio.so, RefFastLioBench.process_scan — the very code
-      bench.py --impl reference times): posterior pose within the north_star's 1e-4 m / 1e-5 rad on every step, same
+      bench.py --impl reference times; its posteriors and counts are stored in tests/golden/config1_ref.npz by
+      tests/golden/make_golden_config1.py): posterior pose within the north_star's 1e-4 m / 1e-5 rad on every step, same
       feats_down_size, same effective-point count to a handful of gate flips (the compiled reference keeps
       std::nth_element's neighbour order, esti_plane's QR is order-sensitive in fp32 — DESIGN.md section 4);
   (b) the plain-C port of iVox on the SAME 10 M-point map: bit-exact neighbour ids for every query of the scan's first
       search, on the shared downsampled cloud.
 
 Both sides start from the same map and register the same scans in the same order, map_incremental included, so step s sees
-the map the steps before it left behind.  LSD_CONFIG1_BLOCKS=2 shrinks the map (2 x 2 blocks) for a dry run under the SIMT
-emulator; the GPU run uses the full 13 x 13."""
+the map the steps before it left behind.  The GPU run uses the full 13 x 13-block map the golden vectors were made on."""
 import os
 
 import numpy as np
@@ -19,6 +19,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 N_STEPS = 6
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "config1_ref.npz")
 
 
 @pytest.mark.parametrize("ref_order", [False, True])
@@ -33,20 +34,16 @@ def test_bench_steps_pose_parity_with_the_compiled_reference(ref_order):
     import lsdreg
     from lsdreg import synth
     from oracle import eskf
-    from oracle import fastlio as FL
     from oracle import oracle as O
-    if not FL.HAVE_REF_FASTLIO:
-        pytest.skip("oracle/_ref/libref_fastlio.so not built (needs /root/reference at build time)")
-    nb = int(os.environ.get("LSD_CONFIG1_BLOCKS", bench.BLOCKS_X))
-    bench.BLOCKS_X = bench.BLOCKS_Y = nb
+    gold = np.load(GOLDEN)
+    assert int(gold["x"].shape[0]) >= N_STEPS
+    nb = bench.BLOCKS_X
     m = synth.block_map(bench.MAP_SEED, nb, nb, bench.SPACING)
-    assert nb != 13 or m.shape[0] > 10_000_000
-    g = lsdreg.LioFrontend(map_log2_lines=25 if nb == 13 else 21, max_scan_points=131072, max_points=100000, async_map_insert=1)
+    assert m.shape[0] > 10_000_000 and m.shape[0] == int(gold["map_points"])
+    g = lsdreg.LioFrontend(map_log2_lines=25, max_scan_points=131072, max_points=100000, async_map_insert=1)
     g.map.insert(m, 0); g.set_next_id(m.shape[0])
     g.set_reference_order(ref_order)
-    ref = FL.RefFastLioBench(capacity=1 << 30, threads=8)
-    ref.add_map_points(m)
-    port = O.OracleIvox(0.5, 18, 1 << 24 if nb == 13 else 1 << 20)
+    port = O.OracleIvox(0.5, 18, 1 << 24)
     port.add(np.ascontiguousarray(m[:, :3]), 0)
     P0 = eskf.init_P()
     worst = np.zeros(2)
@@ -64,8 +61,9 @@ def test_bench_steps_pose_parity_with_the_compiled_reference(ref_order):
             assert (mt["idx"][found] == oi[found]).all()
             assert (mt["idx"][~found] == -1).all()
         x, P, info = g.scan(scan, prior.to_vec(), P0)
-        xr, Pr, n_down_ref = ref.process_scan(scan, prior, P0)
-        c = ref.counts()
+        xr, Pr = eskf.State.from_vec(gold["x"][s]), gold["P"][s]
+        n_down_ref, *cnt = (int(v) for v in gold["counts"][s])
+        c = dict(zip(("n_down", "n_eff", "degenerate", "map_cells"), cnt))
         assert info["status"] == lsdreg.OK and info["n_down"] == n_down_ref == c["n_down"], (s, info, c)
         assert abs(info["n_eff"] - c["n_eff"]) <= (0 if ref_order else max(3, c["n_eff"] // 500)), (s, info["n_eff"], c["n_eff"])
         assert info["degenerate"] == c["degenerate"] == 0

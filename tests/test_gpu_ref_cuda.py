@@ -1,5 +1,5 @@
 """GPU pin of the NDT path against the COMPILED reference CUDA matcher (fast_gicp::NDTCuda / NDTCudaCore recompiled
-for sm_100a: oracle/ref_cuda.cu -> oracle/_ref/libref_cuda.so).  Two properties of the reference bound how tightly it
+for sm_90a: oracle/ref_cuda.cu -> oracle/_ref/libref_cuda.so).  Two properties of the reference bound how tightly it
 can be matched: (1) its voxel hash accepts a table in which up to 1 % of the POINTS found no bucket within 10 probes and
 silently drops their voxels (gaussian_voxelmap.cu:37-52,283-288) — which ones depends on the order of the atomics —
 whereas this library (and the CPU restatement) keep every voxel; (2) it accumulates voxel moments with fp32 atomicAdd in
@@ -59,7 +59,7 @@ HAVE_VFE = os.path.exists(os.path.join(os.path.dirname(os.path.dirname(os.path.a
 @pytest.mark.skipif(not HAVE_VFE, reason="oracle/_ref/libref_vfe.so not built (needs /root/reference + nvcc)")
 @pytest.mark.parametrize("frames", [1, 4])
 def test_voxelizer_matches_compiled_reference_kernels(frames):
-    """lsd_vfe_* against the reference's own Preprocess / Voxelization kernels (recompiled for sm_100a).  The reference
+    """lsd_vfe_* against the reference's own Preprocess / Voxelization kernels (recompiled for sm_90a).  The reference
     assigns voxel rows and point slots in atomic order, so the comparison is per voxel KEY: same window, same voxel set,
     and — for every voxel that holds no more points than the cap, where the reference is deterministic — the same fp16
     features up to the fp32 summation order (1 fp16 ulp)."""

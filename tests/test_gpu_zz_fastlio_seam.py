@@ -10,7 +10,7 @@ restated pipeline itself ends 8e-4 m from the compiled reference after ten updat
 bar is therefore a plumbing bar: 5e-3 m / 1e-3 rad after ten updates, covariance within 15 % of sigma_i sigma_j.  fastlio_odometry / fastlio_state are checked against the filter state they are read from.
 
 STATUS: written after this round's GPU budget was spent — never run on a GPU; the seam's host side IS covered on the CPU
-(tests/test_fastlio_seam_host.py).  Passed on B200 at the end of round 1.  Runs in a subprocess.
+(tests/test_fastlio_seam_host.py).  Runs in a subprocess.
 """
 import os
 import subprocess

@@ -5,7 +5,7 @@ iterates and hands its buffers to the scan that adopts it.  For both: a scan str
 covariance, Nearest_Points ids, downsampled scan, map contents — with and without stale rows, and with the double-buffered
 ingest (a copy-stream event between two PDL launches).
 
-Both are ON by default since round 2 (this test passed on B200 at the end of round 1); it stays as the bit-identity
+Both are ON by default since round 2; it stays as the bit-identity
 guard of the default path against the plain-launch path.  Runs in a subprocess (its own CUDA context).
 """
 import os

@@ -3,7 +3,7 @@
   * fast_gicp::FastVGICP, the CPU/OpenMP class (fast_vgicp_impl.hpp, double precision) compiled unmodified into
     oracle/_ref/libref_reg.so — what registrations.cpp:56-66 selects on a build without CUDA, and what the product's
     VGICP follows;
-  * fast_gicp::FastVGICPCuda over FastVGICPCudaCore recompiled for sm_100a (oracle/ref_cuda_vgicp.cu ->
+  * fast_gicp::FastVGICPCuda over FastVGICPCudaCore recompiled for sm_90a (oracle/ref_cuda_vgicp.cu ->
     oracle/_ref/libref_cuda_vgicp.so) — what registrations.cpp:43-55 selects with USE_VGICP_CUDA.
 
 Round 1 compared the product with the CUDA variant only, at 3 %, and failed (H off by 11 % on one diagonal entry, cost by

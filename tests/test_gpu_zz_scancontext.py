@@ -4,8 +4,8 @@ golden vectors (tests/golden/scancontext_ref.npz, produced by the compiled refer
 and pair distances bit-exact (same reduction order; 1e-12 would be the fallback bar if the device's atan / division ever
 differed in the last bit, which would show up here as a flipped bin); shifts, candidate lists and matches identical.
 
-The kernels' arithmetic (csrc/sc_math.h) is also pinned on the CPU (tests/sc_host_harness.cpp).  Passed on B200 at the end of
-round 1.  Runs in a subprocess.
+The kernels' arithmetic (csrc/sc_math.h) is also pinned on the CPU (tests/sc_host_harness.cpp).  Runs in a
+subprocess.
 """
 import os
 import subprocess

@@ -3,7 +3,7 @@
 IMU initialisation, the seeding scan, NEARBY74 -> NEARBY18, flg_EKF_inited, ten updates with map_incremental, WITH the
 reference's stale Nearest_Points rows (lsd_lio_set_stale_rows).
 
-Passed on B200 at the end of round 1; the stale rows are the product's default since round 2.  Runs in a subprocess.
+The stale rows are the product's default since round 2.  Runs in a subprocess.
 """
 import os
 import subprocess

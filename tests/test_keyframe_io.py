@@ -1,11 +1,10 @@
 """Key-frame files (SURVEY.md section 8f row N3, the on-disk format): lsd_keyframe_save / lsd_keyframe_load and the pybind
 `dump_keyframe` against the reference's own KeyFrame::save / loadOdom / loadPcd compiled unmodified (oracle/ref_keyframe.cpp
--> oracle/_ref/libref_keyframe.so) and against the PCD reader the reference vendors (third_party/pypcd.py).  Host-only
-code: runs without a GPU."""
+-> oracle/_ref/libref_keyframe.so) and against what the PCD reader the reference vendors (third_party/pypcd.py) parsed from
+our file (stored under tests/golden).  Host-only code: runs without a GPU."""
 import ctypes as C
 import os
 import sys
-import types
 
 import numpy as np
 import pytest
@@ -131,27 +130,37 @@ def test_pybind_dump_keyframe_writes_the_same_files(tmp_path):
         assert (a / f).read_bytes() == (b / f).read_bytes()
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/third_party/pypcd.py"), reason="reference tree absent")
+PYPCD_SEED, PYPCD_POINTS = 8, 777
+PYPCD_GOLDEN = os.path.join(_HERE, "golden", "pypcd_keyframe.npz")
+
+
+def _read_pcd(path):
+    """Header fields and binary columns of a DATA binary PCD file."""
+    raw = open(path, "rb").read()
+    head, body = raw.split(b"DATA binary\n", 1)
+    h = {}
+    for line in head.decode("ascii").splitlines():
+        if line and not line.startswith("#"):
+            k, *v = line.split()
+            h[k] = v
+    dt = np.dtype([(f, {"F": "<f", "I": "<i", "U": "<u"}[t] + sz) for f, t, sz in zip(h["FIELDS"], h["TYPE"], h["SIZE"])])
+    return h, np.frombuffer(body, dt, count=int(h["POINTS"][0]))
+
+
 def test_cloud_pcd_is_read_by_the_reference_s_vendored_pcd_reader(tmp_path):
-    """third_party/pypcd.py is the PCD reader the reference ships for its Python tools; lzf (only needed for compressed
-    files) is not installed here and is stubbed, and numpy 2 dropped the binary mode of np.fromstring the reader was written
-    against, so that one call is routed to np.frombuffer."""
-    sys.modules.setdefault("lzf", types.ModuleType("lzf"))
-    sys.path.insert(0, "/root/reference/third_party")
-    try:
-        import pypcd
-    finally:
-        sys.path.remove("/root/reference/third_party")
-    rng = np.random.default_rng(8)
-    pts = _cloud(rng, 777)
+    """third_party/pypcd.py is the PCD reader the reference ships for its Python tools.  What it parsed from the file this
+    library writes for the same seeded key frame is stored in tests/golden/pypcd_keyframe.npz (tests/golden/make_golden_pypcd.py);
+    the file written now must carry the same header and the same columns."""
+    g = np.load(PYPCD_GOLDEN)
+    pts = _cloud(np.random.default_rng(PYPCD_SEED), PYPCD_POINTS)
     d = tmp_path / "kf"; d.mkdir()
     lsdreg.keyframe_save(str(d), 5, 1, pts, np.eye(4))
-    real = np.fromstring
-    pypcd.np.fromstring = lambda buf, dtype=float, **kw: np.frombuffer(buf, dtype=dtype)
-    try:
-        pc = pypcd.PointCloud.from_path(str(d / "cloud.pcd"))
-    finally:
-        pypcd.np.fromstring = real
-    assert pc.points == 777 and list(pc.fields) == ["x", "y", "z", "intensity"]
-    np.testing.assert_array_equal(pc.pc_data["x"], pts[:, 0]); np.testing.assert_array_equal(pc.pc_data["z"], pts[:, 2])
-    np.testing.assert_array_equal(pc.pc_data["intensity"], pts[:, 3] * np.float32(255.0))
+    h, rows = _read_pcd(d / "cloud.pcd")
+    assert int(g["points"]) == PYPCD_POINTS and list(g["fields"]) == ["x", "y", "z", "intensity"] and str(g["data"]) == "binary"
+    assert h["FIELDS"] == list(g["fields"]) and h["SIZE"] == [str(v) for v in g["size"]] and h["TYPE"] == list(g["type"])
+    assert h["COUNT"] == [str(v) for v in g["count"]]
+    assert (int(h["WIDTH"][0]), int(h["HEIGHT"][0]), int(h["POINTS"][0])) == (int(g["width"]), int(g["height"]), int(g["points"]))
+    for f in ("x", "z", "intensity"):
+        np.testing.assert_array_equal(rows[f], g[f])
+    np.testing.assert_array_equal(g["x"], pts[:, 0]); np.testing.assert_array_equal(g["z"], pts[:, 2])
+    np.testing.assert_array_equal(g["intensity"], pts[:, 3] * np.float32(255.0))

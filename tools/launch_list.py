@@ -1,6 +1,6 @@
 """Condense an `ncu --metrics gpu__time_duration.sum --csv --log-file X.csv` launch list into per-kernel count / total / share.
 
-    python tools/launch_list.py gpurun_out/r02a_launches.csv > profiles/r02a_launches_summary.txt
+    python tools/launch_list.py launches.csv > launches_summary.txt
 """
 import csv
 import sys

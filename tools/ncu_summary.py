@@ -2,7 +2,7 @@
 into the dozen numbers the design notes quote: duration, DRAM bytes and rate, instructions per work item, issue utilisation,
 occupancy, lanes active per instruction, L2 hit rate, registers, top stall reasons.
 
-    python tools/ncu_summary.py profiles/r01k_knn_thread_ncu_raw.csv [--items 1048576] [--alg-bytes 680]
+    python tools/ncu_summary.py knn_thread_ncu_raw.csv [--items 1048576] [--alg-bytes 680]
 """
 import csv
 import io

@@ -1,4 +1,4 @@
-"""Head-to-head on one GPU: the reference's CUDA NDT (recompiled for sm_100a, oracle/_ref/libref_cuda.so) against
+"""Head-to-head on one GPU: the reference's CUDA NDT (recompiled for sm_90a, oracle/_ref/libref_cuda.so) against
 liblsdreg, same clouds: agreement of one linearisation and wall time of target build / cost evaluation / align."""
 import json
 import os
@@ -32,7 +32,7 @@ def t_ms(f, n=1):
 out = dict(map_points=int(m.shape[0]), scan_points=int(scan.shape[0]))
 g = lsdreg.Matcher("NDT_CUDA")
 r = RefNdtCuda(1.0, 7)
-for name, mm in (("lsdreg", g), ("reference_cuda_sm100a", r)):
+for name, mm in (("lsdreg", g), ("reference_cuda_sm90a", r)):
     mm.set_target(m[:1000]); mm.set_source(scan[:1000])                       # warm-up (module load, allocator)
     tb = min(t_ms(lambda: mm.set_target(m))[0] for _ in range(3))         # best of 3: allocator growth lands in the first call
     ts = min(t_ms(lambda: mm.set_source(scan))[0] for _ in range(3))
@@ -57,7 +57,7 @@ for f in range(8):
 M = np.eye(4, dtype=np.float32); M[:3, 3] = [0.8, 0.1, 0.0]
 vg, vr = lsdreg.Voxelizer(max_frame_num=4, unordered_ids=1), RefVoxelizer(max_frame_num=4)   # same contract as the reference: ids in atomic order
 vfe = {}
-for name, v in (("lsdreg", vg), ("reference_cuda_sm100a", vr)):
+for name, v in (("lsdreg", vg), ("reference_cuda_sm90a", vr)):
     for f in range(4):
         v.accumulate(frames[f], M)
     v.voxelize(True)

@@ -3,6 +3,7 @@
   config[2]  NDT scan-to-map: 100 k-pt scan vs a 50 M-pt map voxelised at 0.5 m
   config[3]  GICP loop-closure batch: submap pairs x 200 k pts (per-GPU share of the 256-pair batch)
   config[4]  detection voxelizer: 200 k pts, 4-frame window
+  loop       loop-closure detection: one new key frame vs C candidates (C = 4, 16, 32), ~30 k pts each
 Prints one JSON object per config with device times (CUDA events via torch on the default stream are
 NOT used: the library runs on its own stream, so wall time around synchronous C-ABI calls is reported)
 and the CPU restatement timed on a bounded sample.
@@ -308,6 +309,95 @@ def vfe(args):
     print(json.dumps(out))
 
 
+def _card():
+    """Card name and power limit, read in the same run (both are part of any number measured on it)."""
+    import subprocess
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=20).stdout.strip().splitlines()
+        name, pl = [x.strip() for x in q[int(os.environ.get("LOCAL_RANK", 0))].split(",")]
+        return dict(card=name, power_limit=pl)
+    except Exception as e:  # the measurement does not depend on it
+        return dict(card="unknown", power_limit="unknown (%s)" % repr(e)[:80])
+
+
+def loop(args):
+    """LoopDetector on one new key frame and C candidates: batched (lsd_loop_detect / lsd_loop_match) against the per-pair
+    lsd_reg loop a user writes without it, and the reference's own CUDA NDT run candidate after candidate where built."""
+    import lsdreg
+    from lsdreg import synth
+    c0 = synth.block_center(0, 0)
+    card = _card()
+    for C in (4, 16, 32):
+        clouds, poses, accum = [], [], []
+        for i in range(C):
+            th = 2 * np.pi * i / C
+            R = synth.rot_from_rpy(0.0, 0.0, th)
+            t = c0 + np.array([8.0 * np.cos(th), 8.0 * np.sin(th), 0.0])
+            clouds.append(synth.scan64(500 + i, 470, R, t))
+            dR, dt = synth.perturb(600 + i, 0.5, 3.0)
+            T = np.eye(4); T[:3, :3] = R @ dR; T[:3, 3] = t + dt
+            poses.append(T); accum.append(2.0 * i)
+        clouds.append(synth.scan64(499, 470, np.eye(3), c0))
+        poses.append(np.eye(4)); poses[-1][:3, 3] = c0; accum.append(2.0 * C + 30.0)
+        P = np.array(poses)
+        new, kfs = C, list(range(C))
+        d = lsdreg.LoopDetector()
+        for c, a in zip(clouds, accum):
+            d.add_keyframe(c, a)
+        cand, G = d.find_candidates(P, kfs, new)
+        assert len(cand) == C
+        # batched: warm up every shape, then time
+        d.match(new, cand, G)
+        match_ms, m = t_ms(lambda: d.match(new, cand, G), args.loop_reps)
+        d.last_edge_accum_distance = 0.0
+        d.detect(P, kfs, [new])
+        def det():
+            d.last_edge_accum_distance = 0.0
+            return d.detect(P, kfs, [new])
+        detect_ms, loops = t_ms(det, args.loop_reps)
+        # serial: one lsd_reg NDT handle, one pair after another (loop_detector.hpp:158-191 written against lsd_reg)
+        g = lsdreg.Matcher("NDT_CUDA")
+        def serial():
+            g.set_target(clouds[new])
+            out = []
+            for k, gk in zip(cand, G):
+                g.set_source(clouds[k])
+                g.align(gk.astype(np.float32))
+                out.append((g.final()[0], g.converged, g.fitness(25.0)))
+            return out
+        serial()
+        l0 = g.stats()["launches"]
+        serial_ms, ser = t_ms(serial, args.loop_reps)
+        serial_launches = (g.stats()["launches"] - l0) / args.loop_reps
+        same = all(np.array_equal(m["final"][i], ser[i][0]) and bool(m["converged"][i]) == ser[i][1] and m["fitness"][i] == ser[i][2]
+                   for i in range(C))
+        out = dict(config="loop detection: 1 new key frame vs %d candidates" % C, candidates=C,
+                   points_per_keyframe=int(np.mean([c.shape[0] for c in clouds])), **card,
+                   batched=dict(detect_ms=detect_ms, match_ms=match_ms, candidates_per_s=C / (match_ms * 1e-3),
+                                match_launches=m["launches"], match_round_trips=m["rounds"] + 1, loops_found=len(loops)),
+                   serial=dict(ms=serial_ms, candidates_per_s=C / (serial_ms * 1e-3), launches=serial_launches,
+                               round_trips=serial_launches),   # every cost / fitness launch of lsd_reg waits for its result
+                   batched_equals_serial=bool(same),
+                   alg_bytes_per_round=float(sum(c.shape[0] for c in clouds[:C]) * (16 + 7 * (8 + 40))))
+        if not args.no_ref_cuda and os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libref_cuda.so")):
+            try:
+                from oracle.reg import RefNdtCuda
+                r = RefNdtCuda(1.0, 7)
+                def ref():
+                    r.set_target(clouds[new])
+                    for k, gk in zip(cand, G):
+                        r.set_source(clouds[k]); r.align(gk)
+                ref()
+                rm, _ = t_ms(ref, args.loop_reps)
+                out["reference_cuda_sm90a"] = dict(ms=rm, candidates_per_s=C / (rm * 1e-3))
+                del r
+            except Exception as e:  # the comparator must never take the measurement down
+                out["reference_cuda_sm90a"] = dict(error=repr(e)[:200])
+        d.close(); g.close()
+        print(json.dumps(out))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="ndt,gicp,vfe")
@@ -317,6 +407,7 @@ if __name__ == "__main__":
     ap.add_argument("--gicp-method", default="FAST_GICP", choices=["FAST_GICP", "FAST_VGICP"])
     ap.add_argument("--gicp-perturb-m", type=float, default=1.0)
     ap.add_argument("--gicp-perturb-deg", type=float, default=5.0)
+    ap.add_argument("--loop-reps", type=int, default=5)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-ref-cuda", action="store_true", help="skip the legs that time the reference's own CUDA NDT / VGICP (oracle/_ref/libref_cuda*.so)")
     a = ap.parse_args()
@@ -328,6 +419,6 @@ if __name__ == "__main__":
         with contextlib.redirect_stdout(buf):
             lsdreg.init(int(os.environ.get("LOCAL_RANK", 0)))
             for w in a.which.split(","):
-                {"ndt": ndt, "gicp": gicp, "vfe": vfe}[w](a)
+                {"ndt": ndt, "gicp": gicp, "vfe": vfe, "loop": loop}[w](a)
     sys.stdout.write(buf.getvalue())
     sys.stdout.flush()

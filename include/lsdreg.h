@@ -377,6 +377,89 @@ lsd_status_t lsd_reg_get_correspondences(lsd_reg_t* r, int32_t* corr_host, int c
 lsd_status_t lsd_reg_stats(lsd_reg_t* r, int* n_voxels, long long* launches);
 
 /* ------------------------------------------------------------------------------------------
+ * Loop-closure detector — replaces hdl_graph_slam::LoopDetector
+ * (slam/backend/hdl_graph_slam/include/hdl_graph_slam/loop_detector.hpp:33-231, called from
+ * hdl_graph_slam_nodelet.cpp:613) and the fitness part of InformationMatrixCalculator
+ * (information_matrix_calculator.cpp:25-47,71-102).  Key-frame clouds (sensor frame) are uploaded once into a
+ * device pool and addressed by slot.  The coarse stage (NDT_CUDA of every candidate against the new key frame,
+ * :148-191) runs all candidates together: one batched cost launch per Levenberg-Marquardt round for the whole
+ * candidate set, each candidate bit-identical to a separate lsd_reg NDT handle on the same pair.  The refinement
+ * (FAST_GICP, max-corr 0.5 m, :193-219) runs on the one best pair through the lsd_reg GICP code.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct lsd_loop lsd_loop_t;
+typedef struct lsd_loop_params {
+  double distance_thresh;                 /* 15.0 m, x-y distance of the graph estimates (loop_detector.hpp:43,129-133) */
+  double accum_distance_thresh;           /* 25.0 m travelled between candidate and new key frame (:44,119-121)        */
+  double distance_from_last_edge_thresh;  /* 15.0 m travelled since the last accepted loop (:45,108-110)              */
+  double distance_new_keyframe_thresh;    /* 2.0 m between the new key frames examined in one detect (:46,78-80)      */
+  double distance_keyframe_thresh;        /* 2.0 m between accepted candidates (:47,123-125)                          */
+  double fitness_score_max_range;         /* 25.0, SQUARED distance as PCL compares it (:49,180,206)                   */
+  double fitness_score_thresh;            /* 1.5 (:50; the coarse gate is 2x this, :193)                              */
+  lsd_reg_params_t coarse;                /* lsd_reg_default_params(LSD_REG_NDT_P2D): "NDT_CUDA", registrations.cpp:107-118;
+                                             max_process_time_us must be 0 (the reference sets no timeout)             */
+  lsd_reg_params_t accurate;              /* LSD_REG_GICP with max_corr_dist = 0.5 (loop_detector.hpp:58-59)           */
+} lsd_loop_params_t;
+
+typedef struct lsd_loop_result {
+  int32_t key1, key2;          /* new key frame slot, matched candidate slot (Loop::key1 / key2)                     */
+  float relpose16[16];         /* registration_accurate->getFinalTransformation(), row-major (:216)                  */
+  double coarse_score, score;  /* best NDT getFitnessScore (:180), final GICP getFitnessScore (:206)                 */
+  double information36[36];    /* calc_information_matrix(key1 cloud, key2 cloud, relpose), row-major               */
+  int32_t n_candidates;        /* candidates the coarse stage matched                                                 */
+} lsd_loop_result_t;
+
+/* What detect decided for each new key frame it was given (no reference counterpart beyond its LOG_INFO lines). */
+#define LSD_LOOP_SKIPPED 0         /* closer than distance_new_keyframe_thresh to the previous one examined (:78-80) */
+#define LSD_LOOP_NO_CANDIDATES 1   /* find_candidates returned nothing (:150-152)                                    */
+#define LSD_LOOP_COARSE_REJECT 2   /* best NDT score above 2 * fitness_score_thresh, or nothing converged (:193-196) */
+#define LSD_LOOP_GICP_DIVERGED 3   /* the refinement did not converge (:202-205)                                     */
+#define LSD_LOOP_GICP_REJECT 4     /* the refined score is above fitness_score_thresh (:206-210)                     */
+#define LSD_LOOP_FOUND 5
+typedef struct lsd_loop_report {
+  int32_t new_slot, decision, n_candidates, best_slot;  /* best_slot: the coarse stage's choice, -1 = none   */
+  double best_score;                                    /* its NDT score (DBL_MAX when nothing converged)   */
+} lsd_loop_report_t;
+
+void lsd_loop_default_params(lsd_loop_params_t* p);
+lsd_status_t lsd_loop_create(lsd_loop_t** out, const lsd_loop_params_t* p);
+lsd_status_t lsd_loop_destroy(lsd_loop_t* h);
+/* KeyFrame (keyframe.hpp:21-41): its cloud (sensor frame, [n,4]) is uploaded once and kept on the device;
+ * accum_distance as KeyFrame::accum_distance.  *slot = 0, 1, 2, ... in call order. */
+lsd_status_t lsd_loop_add_keyframe(lsd_loop_t* h, const float* xyzi_host, int n, double accum_distance, int32_t* slot);
+/* LoopDetector::detect (:69-91).  poses16 = the current graph estimate of EVERY slot ([n_slots,16], double, row-major,
+ * node->estimate()); keyframes / new_keyframes = slots in the order of the reference's vector / deque.  Writes up to
+ * cap loops; *n_loops = loops found (may exceed cap).  last_edge_accum_distance persists across calls (:60,216). */
+lsd_status_t lsd_loop_detect(lsd_loop_t* h, const double* poses16, const int32_t* keyframes, int n_kf,
+                             const int32_t* new_keyframes, int n_new, lsd_loop_result_t* out, int cap, int* n_loops);
+/* Per new key frame of the last lsd_loop_detect, in order: what was decided (LSD_LOOP_*).  out may be NULL. */
+lsd_status_t lsd_loop_last_reports(lsd_loop_t* h, lsd_loop_report_t* out, int cap, int* n);
+/* last_edge_accum_distance (:216) of the handle: read (get != 0) or set. */
+lsd_status_t lsd_loop_last_edge(lsd_loop_t* h, double* value, int get);
+/* find_candidates (:106-140) and the initial guess of each candidate (:165-173: both rotations normalised through a
+ * quaternion, new^-1 * candidate in double, cast to float, element (2,3) zeroed; returned as double).  Pure host: works
+ * without a device.  accum = KeyFrame::accum_distance of every slot.  *n_cand = candidates found (may exceed cap). */
+lsd_status_t lsd_loop_find_candidates(const lsd_loop_params_t* p, double last_edge_accum_distance, const double* poses16,
+                                      const double* accum, const int32_t* keyframes, int n_kf, int32_t new_slot,
+                                      int32_t* cand_out, double* guesses16_out, int cap, int* n_cand);
+/* Parity tap: the coarse stage alone (:158-191 without the selection) for an explicit candidate list against target_slot.
+ * Per candidate: final NDT pose (double [n,16]), converged, iterations (hasConverged / the LM iteration count of
+ * lsd_reg_align), getFitnessScore(fitness_score_max_range) at that pose.  Any output may be NULL.  *launches / *rounds:
+ * kernel launches and host round trips (one batched cost evaluation each) the call used. */
+lsd_status_t lsd_loop_match(lsd_loop_t* h, int32_t target_slot, const int32_t* cand, const double* guesses16, int n,
+                            double* final16, int32_t* converged, int32_t* iterations, double* fitness, long long* launches,
+                            int* rounds);
+/* The LM iteration log of candidate i of the last lsd_loop_match, same layout as lsd_reg_iteration_log. */
+lsd_status_t lsd_loop_iteration_log(lsd_loop_t* h, int i, double* out4_per_iter, int cap_iters, int* n_iters);
+/* calc_fitness_score(target cloud, source cloud, T, max_range) (information_matrix_calculator.cpp:71-102): mean squared
+ * distance of every transformed source point to its nearest target point, however far (max_range = DBL_MAX counts them
+ * all).  T16 is applied in float, as pcl::transformPointCloud does. */
+lsd_status_t lsd_loop_fitness(lsd_loop_t* h, int32_t target_slot, int32_t source_slot, const float* T16, double max_range,
+                              double* score, int* n_counted);
+/* InformationMatrixCalculator::calc_information_matrix(fitness_score) (:49-62): identity / w_x (translation), / w_q
+ * (rotation), w_* = weight() stored in float.  Pure host. */
+void lsd_loop_information_matrix(double fitness_score, double* information36);
+
+/* ------------------------------------------------------------------------------------------
  * Detection voxelizer (config 5) — replaces sensor_driver/inference/voxelize:
  * Preprocess::forward (preprocess_kernel.cu:56-101: sliding window of max_frame_num frames, older frames
  * re-projected by a 3x4 motion, time channel + 0.1) and Voxelization::forward (voxelization_kernel.cu:

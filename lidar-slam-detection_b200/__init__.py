@@ -9,5 +9,7 @@ from .capi import (  # noqa: F401
     ERR_CAPACITY, ERR_CUDA, ERR_GRID_OVERFLOW, ERR_INVALID, ERR_NO_DEVICE, MAP_SEEDED, NO_EFFECTIVE_POINTS, OK,
     SCAN_TOO_SMALL, MAP_SATURATED, STENCIL_CENTER, STENCIL_EXACT, STENCIL_NEARBY6, STENCIL_NEARBY18, STENCIL_NEARBY26,
     STENCIL_NEARBY74, HashVoxelMap, Matcher, Voxelizer, eskf_update_table, LioFrontend, LsdError, VoxelGrid, init, init_cov, lib, make_state,
-    state_boxminus, state_boxplus, ImuProcess, eskf_predict, IMU_INITIALIZING, keyframe_filter, LocalMap, LOCALMAP_NONE, keyframe_save, keyframe_load, ERR_IO, ScanContext, FastLio)
+    state_boxminus, state_boxplus, ImuProcess, eskf_predict, IMU_INITIALIZING, keyframe_filter, LocalMap, LOCALMAP_NONE, keyframe_save, keyframe_load, ERR_IO, ScanContext, FastLio,
+    LoopDetector, find_loop_candidates, loop_information_matrix, LOOP_SKIPPED, LOOP_NO_CANDIDATES, LOOP_COARSE_REJECT,
+    LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND)
 from . import capi  # noqa: F401

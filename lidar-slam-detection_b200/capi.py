@@ -53,6 +53,27 @@ class RegParams(C.Structure):
 REG_NDT_P2D, REG_GICP, REG_VGICP = 0, 1, 2
 
 
+class LoopParams(C.Structure):
+    _fields_ = [("distance_thresh", C.c_double), ("accum_distance_thresh", C.c_double),
+                ("distance_from_last_edge_thresh", C.c_double), ("distance_new_keyframe_thresh", C.c_double),
+                ("distance_keyframe_thresh", C.c_double), ("fitness_score_max_range", C.c_double),
+                ("fitness_score_thresh", C.c_double), ("coarse", RegParams), ("accurate", RegParams)]
+
+
+class LoopResult(C.Structure):
+    _fields_ = [("key1", C.c_int32), ("key2", C.c_int32), ("relpose16", C.c_float * 16), ("coarse_score", C.c_double),
+                ("score", C.c_double), ("information36", C.c_double * 36), ("n_candidates", C.c_int32)]
+
+
+class LoopReport(C.Structure):
+    _fields_ = [("new_slot", C.c_int32), ("decision", C.c_int32), ("n_candidates", C.c_int32), ("best_slot", C.c_int32),
+                ("best_score", C.c_double)]
+
+
+# what LoopDetector.detect decided for each new key frame (LSD_LOOP_*)
+LOOP_SKIPPED, LOOP_NO_CANDIDATES, LOOP_COARSE_REJECT, LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND = range(6)
+
+
 class ImuParams(C.Structure):
     _fields_ = [("ext_R", C.c_double * 9), ("ext_t", C.c_double * 3), ("gyr_cov", C.c_double), ("acc_cov", C.c_double),
                 ("b_gyr_cov", C.c_double), ("b_acc_cov", C.c_double), ("undistort", C.c_int)]
@@ -143,6 +164,18 @@ SIGNATURES = [
     ("lsd_reg_iteration_log", _i, [_vp, _vp, _i, _pi]),
     ("lsd_reg_shard_export", _i, [_vp, _i, _i, _i, _vp]),
     ("lsd_reg_shard_connect", _i, [_vp, _vp]),
+    ("lsd_loop_default_params", None, [C.POINTER(LoopParams)]),
+    ("lsd_loop_create", _i, [_pp, C.POINTER(LoopParams)]),
+    ("lsd_loop_destroy", _i, [_vp]),
+    ("lsd_loop_add_keyframe", _i, [_vp, _vp, _i, _d, C.POINTER(C.c_int32)]),
+    ("lsd_loop_detect", _i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _i, _pi]),
+    ("lsd_loop_last_reports", _i, [_vp, _vp, _i, _pi]),
+    ("lsd_loop_last_edge", _i, [_vp, C.POINTER(_d), _i]),
+    ("lsd_loop_find_candidates", _i, [C.POINTER(LoopParams), _d, _vp, _vp, _vp, _i, C.c_int32, _vp, _vp, _i, _pi]),
+    ("lsd_loop_match", _i, [_vp, C.c_int32, _vp, _vp, _i, _vp, _vp, _vp, _vp, C.POINTER(C.c_longlong), _pi]),
+    ("lsd_loop_iteration_log", _i, [_vp, _i, _vp, _i, _pi]),
+    ("lsd_loop_fitness", _i, [_vp, C.c_int32, C.c_int32, _vp, _d, C.POINTER(_d), _pi]),
+    ("lsd_loop_information_matrix", None, [_d, _vp]),
     ("lsd_vfe_default_params", None, [C.POINTER(VfeParams)]),
     ("lsd_vfe_create", _i, [_pp, C.POINTER(VfeParams)]),
     ("lsd_vfe_destroy", _i, [_vp]),
@@ -556,6 +589,145 @@ class Matcher:
         nv, ln = C.c_int(), C.c_longlong()
         check(lib.lsd_reg_stats(self.h, C.byref(nv), C.byref(ln)))
         return dict(n_voxels=nv.value, launches=ln.value)
+
+
+def _loop_params(**kw) -> LoopParams:
+    p = LoopParams()
+    lib.lsd_loop_default_params(C.byref(p))
+    for k, v in kw.items():
+        if k in ("coarse", "accurate"):          # dict of lsd_reg_params_t fields
+            for kk, vv in v.items():
+                if not hasattr(p.coarse, kk):
+                    raise TypeError(f"unknown matcher parameter {kk}")
+                setattr(getattr(p, k), kk, vv)
+        elif hasattr(p, k):
+            setattr(p, k, v)
+        else:
+            raise TypeError(f"unknown loop-detector parameter {k}")
+    return p
+
+
+def _slots(a) -> np.ndarray:
+    return np.ascontiguousarray(a, np.int32).reshape(-1)
+
+
+def _poses(a) -> np.ndarray:
+    a = np.ascontiguousarray(a, np.float64)
+    if a.ndim != 3 or a.shape[1:] != (4, 4):
+        raise ValueError("poses must be float64 [n_slots, 4, 4]")
+    return a
+
+
+class LoopDetector:
+    """hdl_graph_slam::LoopDetector (loop_detector.hpp) on the device: key frames are added once (their clouds stay in
+    device memory, addressed by slot); detect() finds candidates, aligns all of them to the new key frame with batched
+    NDT, refines the best with GICP and returns the loops with their information matrices."""
+
+    def __init__(self, **kw):
+        self.h = None
+        self.params = _loop_params(**kw)
+        self.h = C.c_void_p()
+        check(lib.lsd_loop_create(C.byref(self.h), C.byref(self.params)))
+        self.accum = []
+
+    def close(self):
+        if self.h:
+            lib.lsd_loop_destroy(self.h)
+        self.h = None
+
+    __del__ = close
+
+    def add_keyframe(self, pts, accum_distance: float) -> int:
+        pts = _f32(pts)
+        slot = C.c_int32()
+        check(lib.lsd_loop_add_keyframe(self.h, _ptr(pts), pts.shape[0], float(accum_distance), C.byref(slot)))
+        self.accum.append(float(accum_distance))
+        return slot.value
+
+    @property
+    def last_edge_accum_distance(self) -> float:
+        v = C.c_double()
+        check(lib.lsd_loop_last_edge(self.h, C.byref(v), 1))
+        return v.value
+
+    @last_edge_accum_distance.setter
+    def last_edge_accum_distance(self, value: float):
+        v = C.c_double(value)
+        check(lib.lsd_loop_last_edge(self.h, C.byref(v), 0))
+
+    def detect(self, poses, keyframes, new_keyframes) -> list[dict]:
+        """poses: graph estimate of every slot [n_slots, 4, 4]; keyframes / new_keyframes: slots.  One dict per loop."""
+        P, kf, nk = _poses(poses), _slots(keyframes), _slots(new_keyframes)
+        cap = max(len(nk), 1)
+        out = (LoopResult * cap)()
+        n = C.c_int()
+        check(lib.lsd_loop_detect(self.h, _ptr(P), _ptr(kf), kf.size, _ptr(nk), nk.size, out, cap, C.byref(n)))
+        return [dict(key1=r.key1, key2=r.key2, relpose=np.array(r.relpose16, np.float32).reshape(4, 4),
+                     coarse_score=r.coarse_score, score=r.score, information=np.array(r.information36).reshape(6, 6),
+                     n_candidates=r.n_candidates) for r in out[:n.value]]
+
+    def reports(self) -> list[dict]:
+        """What the last detect() decided for each new key frame (decision: LOOP_*)."""
+        n = C.c_int()
+        check(lib.lsd_loop_last_reports(self.h, None, 0, C.byref(n)))
+        out = (LoopReport * max(n.value, 1))()
+        check(lib.lsd_loop_last_reports(self.h, out, n.value, C.byref(n)))
+        return [dict(new_slot=r.new_slot, decision=r.decision, n_candidates=r.n_candidates, best_slot=r.best_slot,
+                     best_score=r.best_score) for r in out[:n.value]]
+
+    def find_candidates(self, poses, keyframes, new_slot: int, last_edge_accum_distance: float | None = None, accum=None):
+        """find_candidates + the initial guesses (pure host).  Returns (slots [c], guesses [c, 4, 4])."""
+        return find_loop_candidates(poses, self.accum if accum is None else accum, keyframes, new_slot,
+                                    self.last_edge_accum_distance if last_edge_accum_distance is None else last_edge_accum_distance,
+                                    params=self.params)
+
+    def match(self, target_slot: int, candidates, guesses) -> dict:
+        """The coarse stage alone for an explicit candidate list (parity tap)."""
+        cand = _slots(candidates)
+        n = cand.size
+        G = np.ascontiguousarray(guesses, np.float64).reshape(n, 4, 4)
+        T = np.zeros((n, 4, 4)); cv = np.zeros(n, np.int32); it = np.zeros(n, np.int32); fit = np.zeros(n)
+        ln, rd = C.c_longlong(), C.c_int()
+        check(lib.lsd_loop_match(self.h, int(target_slot), _ptr(cand), _ptr(G), n, _ptr(T), _ptr(cv), _ptr(it), _ptr(fit),
+                                 C.byref(ln), C.byref(rd)))
+        logs = []
+        for i in range(n):
+            m = C.c_int()
+            check(lib.lsd_loop_iteration_log(self.h, i, None, 0, C.byref(m)))
+            lg = np.zeros((max(m.value, 1), 4))
+            check(lib.lsd_loop_iteration_log(self.h, i, _ptr(lg), m.value, C.byref(m)))
+            logs.append(lg[:m.value])
+        return dict(final=T, converged=cv.astype(bool), iterations=it, fitness=fit, launches=ln.value, rounds=rd.value,
+                    iteration_logs=logs)
+
+    def fitness(self, target_slot: int, source_slot: int, T, max_range: float = 1.7976931348623157e308):
+        """calc_fitness_score(target, source, T, max_range): (score, points counted)."""
+        Tf = np.ascontiguousarray(T, np.float32)
+        sc, n = C.c_double(), C.c_int()
+        check(lib.lsd_loop_fitness(self.h, int(target_slot), int(source_slot), _ptr(Tf), max_range, C.byref(sc), C.byref(n)))
+        return sc.value, n.value
+
+
+def find_loop_candidates(poses, accum, keyframes, new_slot: int, last_edge_accum_distance: float = 0.0, params=None, **kw):
+    """LoopDetector::find_candidates and the guesses of matching() (pure host, no device needed)."""
+    p = params if params is not None else _loop_params(**kw)
+    P, kf = _poses(poses), _slots(keyframes)
+    acc = np.ascontiguousarray(accum, np.float64)
+    if acc.size != P.shape[0] or not 0 <= new_slot < P.shape[0]:
+        raise ValueError("one accum_distance and one pose per slot")
+    cand = np.zeros(max(kf.size, 1), np.int32)
+    G = np.zeros((max(kf.size, 1), 4, 4))
+    n = C.c_int()
+    check(lib.lsd_loop_find_candidates(C.byref(p), float(last_edge_accum_distance), _ptr(P), _ptr(acc), _ptr(kf), kf.size,
+                                       int(new_slot), _ptr(cand), _ptr(G), cand.size, C.byref(n)))
+    return cand[:n.value].copy(), G[:n.value].copy()
+
+
+def loop_information_matrix(fitness_score: float) -> np.ndarray:
+    """InformationMatrixCalculator::calc_information_matrix for a given fitness score (pure host)."""
+    out = np.zeros((6, 6))
+    lib.lsd_loop_information_matrix(float(fitness_score), _ptr(out))
+    return out
 
 
 def eskf_update_table(state, P, HTH, HTh, n_eff, R=0.001, max_iterations=4, eps=0.001, literal=False, converge_log=None):

@@ -4,6 +4,7 @@
 #include "voxelgrid.cu"
 #include "lio.cu"
 #include "reg.cu"
+#include "loop.cu"
 #include "vfe.cu"
 #include "imu.cu"
 #include "filters.cu"

@@ -137,6 +137,67 @@ __device__ __forceinline__ int ndt_lookup(const NdtView& v, int x, int y, int z)
 struct Pose34f { float R[9], t[3]; };
 __constant__ signed char c_ndt_off7[7][3] = {{0,0,0},{1,0,0},{-1,0,0},{0,1,0},{0,-1,0},{0,0,1},{0,0,-1}};
 
+// One source point of an NDT cost evaluation (find_voxel_correspondences + p2d_ndt_compute_derivatives).  `corr` points at
+// the [n_off, n] correspondence slots of this cloud.  Shared by the single-pair kernel below (compile-time flags) and the
+// batched loop-closure kernel (loop.cu, flags per candidate): the same expressions, so the same bits.
+__device__ __forceinline__ void ndt_point(const NdtView& v, const float4 a, int i, int n, int n_off, const Pose34f& lin,
+                                          const Pose34f& ev, int* __restrict__ corr, bool update, bool deriv, double (&vals)[29]) {
+  const float k_sq = v.res * v.res;
+  const float tx = ev.R[0] * a.x + ev.R[1] * a.y + ev.R[2] * a.z + ev.t[0];
+  const float ty = ev.R[3] * a.x + ev.R[4] * a.y + ev.R[5] * a.z + ev.t[1];
+  const float tz = ev.R[6] * a.x + ev.R[7] * a.y + ev.R[8] * a.z + ev.t[2];
+  int3 c = make_int3(0, 0, 0);
+  if (update) {
+    const float lx = lin.R[0] * a.x + lin.R[1] * a.y + lin.R[2] * a.z + lin.t[0];
+    const float ly = lin.R[3] * a.x + lin.R[4] * a.y + lin.R[5] * a.z + lin.t[1];
+    const float lz = lin.R[6] * a.x + lin.R[7] * a.y + lin.R[8] * a.z + lin.t[2];
+    c = ndt_coord(lx, ly, lz, v.res);
+  }
+#pragma unroll 1
+  for (int o = 0; o < n_off; o++) {
+    int slot;
+    if (update) {
+      int ox, oy, oz;
+      if (n_off == 27) { ox = o / 9 - 1; oy = (o / 3) % 3 - 1; oz = o % 3 - 1; }
+      else { ox = c_ndt_off7[o][0]; oy = c_ndt_off7[o][1]; oz = c_ndt_off7[o][2]; }
+      slot = ndt_lookup(v, c.x + ox, c.y + oy, c.z + oz);
+      corr[(size_t)o * n + i] = slot;
+    } else {
+      slot = corr[(size_t)o * n + i];
+    }
+    if (slot < 0) continue;
+    vals[28] += 1.0;  // correspondences found
+    const NdtLine* ln = v.lines + slot;
+    const float4 h = __ldg(reinterpret_cast<const float4*>(ln) + 0);          // key lo/hi, n, mean.x
+    const float4 g = __ldg(reinterpret_cast<const float4*>(ln) + 1);          // mean.y, mean.z, nrm.x, nrm.y
+    const float nz = __ldg(reinterpret_cast<const float*>(ln) + 8);
+    if (__float_as_int(h.z) <= 6) continue;                                   // ndt_compute_derivatives.cu:62-64
+    const float mx = h.w, my = g.x, mz = g.y, nx = g.z, ny = g.w;
+    const float ex = mx - tx, ey = my - ty, ez = mz - tz;
+    const float ne = nx * ex + ny * ey + nz * ez;
+    const float cx = ex + 999.0f * nx * ne, cy = ey + 999.0f * ny * ne, cz = ez + 999.0f * nz * ne;  // C^-1 e
+    const float xn = sqrtf(ex * ex + ey * ey + ez * ez);
+    const float w = k_sq / (k_sq + xn * xn);                                   // cauchy
+    vals[27] += (double)(w * (ex * cx + ey * cy + ez * cz));
+    if (deriv) {
+      const float J[3][6] = {{0.f, -tz, ty, -1.f, 0.f, 0.f}, {tz, 0.f, -tx, 0.f, -1.f, 0.f}, {-ty, tx, 0.f, 0.f, 0.f, -1.f}};
+      float M[3][6];
+#pragma unroll
+      for (int cc = 0; cc < 6; cc++) {
+        const float nj = nx * J[0][cc] + ny * J[1][cc] + nz * J[2][cc];
+        M[0][cc] = J[0][cc] + 999.0f * nx * nj; M[1][cc] = J[1][cc] + 999.0f * ny * nj; M[2][cc] = J[2][cc] + 999.0f * nz * nj;
+      }
+      int q = 0;
+#pragma unroll
+      for (int p = 0; p < 6; p++) {
+#pragma unroll
+        for (int r = p; r < 6; r++) vals[q++] += (double)(w * (J[0][p] * M[0][r] + J[1][p] * M[1][r] + J[2][p] * M[2][r]));
+        vals[21 + p] += (double)(w * (J[0][p] * cx + J[1][p] * cy + J[2][p] * cz));
+      }
+    }
+  }
+}
+
 // One NDT cost evaluation (find_voxel_correspondences + p2d_ndt_compute_derivatives + sum).
 // UPDATE: look the correspondences up at the linearisation pose and store them; else reuse.
 // DERIV: accumulate H (21) and b (6) besides the error.
@@ -148,64 +209,9 @@ __global__ void __launch_bounds__(256) ndt_cost_kernel(NdtView v, const float4* 
   double vals[29];
 #pragma unroll
   for (int j = 0; j < 29; j++) vals[j] = 0.0;
-  const float k_sq = v.res * v.res;
 #pragma unroll 1
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 a = __ldg(src + i);
-    const float tx = ev.R[0] * a.x + ev.R[1] * a.y + ev.R[2] * a.z + ev.t[0];
-    const float ty = ev.R[3] * a.x + ev.R[4] * a.y + ev.R[5] * a.z + ev.t[1];
-    const float tz = ev.R[6] * a.x + ev.R[7] * a.y + ev.R[8] * a.z + ev.t[2];
-    int3 c = make_int3(0, 0, 0);
-    if (UPDATE) {
-      const float lx = lin.R[0] * a.x + lin.R[1] * a.y + lin.R[2] * a.z + lin.t[0];
-      const float ly = lin.R[3] * a.x + lin.R[4] * a.y + lin.R[5] * a.z + lin.t[1];
-      const float lz = lin.R[6] * a.x + lin.R[7] * a.y + lin.R[8] * a.z + lin.t[2];
-      c = ndt_coord(lx, ly, lz, v.res);
-    }
-#pragma unroll 1
-    for (int o = 0; o < n_off; o++) {
-      int slot;
-      if (UPDATE) {
-        int ox, oy, oz;
-        if (n_off == 27) { ox = o / 9 - 1; oy = (o / 3) % 3 - 1; oz = o % 3 - 1; }
-        else { ox = c_ndt_off7[o][0]; oy = c_ndt_off7[o][1]; oz = c_ndt_off7[o][2]; }
-        slot = ndt_lookup(v, c.x + ox, c.y + oy, c.z + oz);
-        corr[(size_t)o * n + i] = slot;
-      } else {
-        slot = corr[(size_t)o * n + i];
-      }
-      if (slot < 0) continue;
-      vals[28] += 1.0;  // correspondences found
-      const NdtLine* ln = v.lines + slot;
-      const float4 h = __ldg(reinterpret_cast<const float4*>(ln) + 0);          // key lo/hi, n, mean.x
-      const float4 g = __ldg(reinterpret_cast<const float4*>(ln) + 1);          // mean.y, mean.z, nrm.x, nrm.y
-      const float nz = __ldg(reinterpret_cast<const float*>(ln) + 8);
-      if (__float_as_int(h.z) <= 6) continue;                                   // ndt_compute_derivatives.cu:62-64
-      const float mx = h.w, my = g.x, mz = g.y, nx = g.z, ny = g.w;
-      const float ex = mx - tx, ey = my - ty, ez = mz - tz;
-      const float ne = nx * ex + ny * ey + nz * ez;
-      const float cx = ex + 999.0f * nx * ne, cy = ey + 999.0f * ny * ne, cz = ez + 999.0f * nz * ne;  // C^-1 e
-      const float xn = sqrtf(ex * ex + ey * ey + ez * ez);
-      const float w = k_sq / (k_sq + xn * xn);                                   // cauchy
-      vals[27] += (double)(w * (ex * cx + ey * cy + ez * cz));
-      if (DERIV) {
-        const float J[3][6] = {{0.f, -tz, ty, -1.f, 0.f, 0.f}, {tz, 0.f, -tx, 0.f, -1.f, 0.f}, {-ty, tx, 0.f, 0.f, 0.f, -1.f}};
-        float M[3][6];
-#pragma unroll
-        for (int cc = 0; cc < 6; cc++) {
-          const float nj = nx * J[0][cc] + ny * J[1][cc] + nz * J[2][cc];
-          M[0][cc] = J[0][cc] + 999.0f * nx * nj; M[1][cc] = J[1][cc] + 999.0f * ny * nj; M[2][cc] = J[2][cc] + 999.0f * nz * nj;
-        }
-        int q = 0;
-#pragma unroll
-        for (int p = 0; p < 6; p++) {
-#pragma unroll
-          for (int r = p; r < 6; r++) vals[q++] += (double)(w * (J[0][p] * M[0][r] + J[1][p] * M[1][r] + J[2][p] * M[2][r]));
-          vals[21 + p] += (double)(w * (J[0][p] * cx + J[1][p] * cy + J[2][p] * cz));
-        }
-      }
-    }
-  }
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    ndt_point(v, __ldg(src + i), i, n, n_off, lin, ev, corr, UPDATE, DERIV, vals);
   block_partials<29>(vals, partials);
   grid_finalize<29>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
@@ -742,17 +748,17 @@ static void T_to_pose(const double* T, Pose34d* d, Pose34f* f) {
   }
 }
 
-// Spin on the sequence number the cost kernel publishes into mapped host memory (acquire: the sums stored before it must
-// not be read ahead of it on hosts that reorder loads; bounded, so a hung kernel becomes an error).
-static lsd_status_t reg_wait(lsd_reg* r, double seq) {
-  const unsigned long long* h = reinterpret_cast<const unsigned long long*>(r->h_result + kResSeq);
+// Spin on the sequence number a reduction kernel publishes into mapped host memory (acquire: the sums stored before it
+// must not be read ahead of it on hosts that reorder loads; bounded, so a hung kernel becomes an error).
+static lsd_status_t wait_seq(const double* h_seq_slot, cudaStream_t stream, double seq) {
+  const unsigned long long* h = reinterpret_cast<const unsigned long long*>(h_seq_slot);
   unsigned long long want;
   memcpy(&want, &seq, 8);
   const auto t0 = std::chrono::steady_clock::now();
   for (unsigned long long spins = 0;; spins++) {
     if (__atomic_load_n(h, __ATOMIC_ACQUIRE) == want) return LSD_OK;
     if ((spins & 0xfff) == 0xfff) {
-      cudaError_t e = cudaStreamQuery(r->stream);
+      cudaError_t e = cudaStreamQuery(stream);
       if (e != cudaSuccess && e != cudaErrorNotReady) return cuda_fail(e, "kernel while waiting for the reduction", __FILE__, __LINE__);
       if (e == cudaSuccess) {
         if (__atomic_load_n(h, __ATOMIC_ACQUIRE) == want) return LSD_OK;
@@ -763,6 +769,7 @@ static lsd_status_t reg_wait(lsd_reg* r, double seq) {
     }
   }
 }
+static lsd_status_t reg_wait(lsd_reg* r, double seq) { return wait_seq(r->h_result + kResSeq, r->stream, seq); }
 
 constexpr int kThreadShapeMin = 16384;  // clouds from this size on use the thread-per-point search kernels
 static int reg_grid(int n) { return std::max(1, std::min((n + 255) / 256, kLioMaxGrid)); }
@@ -886,11 +893,11 @@ static double rot_angle(const double* T) {
   if (qw < 0) qw = -qw;  // AngleAxis(Quaternion): angle = 2 atan2(|vec|, |w|)
   return 2.0 * atan2(n, qw);
 }
-static bool is_converged(const lsd_reg* r, const double* delta, double scale) {  // lsq_registration_impl.hpp:112-131
+static bool is_converged(const lsd_reg_params_t& p, const double* delta, double scale) {  // lsq_registration_impl.hpp:112-131
   const double Rdeg = rot_angle(delta) / M_PI * 180.0;
-  const double r_delta = 1.0 / (r->p.rotation_epsilon_deg * scale) * Rdeg;
+  const double r_delta = 1.0 / (p.rotation_epsilon_deg * scale) * Rdeg;
   double t_delta = 0;
-  for (int i = 0; i < 3; i++) t_delta = std::max(t_delta, fabs(delta[4 * i + 3]) / (r->p.transformation_epsilon * scale));
+  for (int i = 0; i < 3; i++) t_delta = std::max(t_delta, fabs(delta[4 * i + 3]) / (p.transformation_epsilon * scale));
   return std::max(r_delta, t_delta) < 1;
 }
 // solve (H + lambda I) d = -b by LDL^T (SPD after damping)
@@ -917,70 +924,133 @@ static bool solve6(const double* H, double lambda, const double* b, double* d) {
   return true;
 }
 
-// LsqRegistration::computeTransformation with step_lm (lsq_registration_impl.hpp:71-109,163-208)
+// LsqRegistration::computeTransformation with step_lm (lsq_registration_impl.hpp:71-109,163-208) as a resumable state:
+// the state names the cost evaluation it needs next (want_T, want_update: linearize with H and b, else compute_error) and
+// lm_feed consumes its result.  lsd_reg_align drives one state to the end; the loop detector (loop.cu) advances a whole
+// candidate set, one batched evaluation per round.  One implementation of the LM rules serves both.
+struct LmState {
+  lsd_reg_params_t p;
+  double x0[16], lambda, nu, H[36], b[6], y0, d[6], delta[16], xi[16], final_H[36];
+  int it, trial;
+  bool stepped, stationary;
+  int converged, iterations;
+  bool done, h_set;                 // h_set: final_H holds the Hessian of an accepted step
+  double want_T[16];
+  bool want_update;
+  std::chrono::steady_clock::time_point clock0;
+  double timeout_ms;
+  std::vector<double> iter_log;     // 4 doubles per outer iteration (lsd_reg_iteration_log)
+};
+
+static void lm_finish(LmState& s) { s.done = true; }
+
+// next LM trial of the current outer iteration, or the end of the iteration when none is left
+static void lm_end_outer(LmState& s);
+static void lm_try_trial(LmState& s) {
+  if (s.trial >= s.p.lm_max_iterations || !solve6(s.H, s.lambda, s.b, s.d)) { s.stepped = false; lm_end_outer(s); return; }
+  se3_exp(s.d, s.delta);
+  mat4_mul(s.delta, s.x0, s.xi);
+  memcpy(s.want_T, s.xi, sizeof(s.xi));
+  s.want_update = false;
+}
+
+static void lm_end_outer(LmState& s) {
+  if (!s.stepped) { lm_finish(s); return; }  // "lm not converged!!"
+  s.converged = is_converged(s.p, s.delta, 1.0) ? 1 : 0;
+  {  // what is_converged looked at (lsd_reg_iteration_log): |t|_inf of the step, its rotation angle, the cost it started from
+    double tm = 0; for (int k = 0; k < 3; k++) tm = std::max(tm, fabs(s.delta[4 * k + 3]));
+    s.iter_log.push_back(tm); s.iter_log.push_back(rot_angle(s.delta) / M_PI * 180.0); s.iter_log.push_back(s.y0); s.iter_log.push_back(s.lambda);
+  }
+  if (s.timeout_ms > 0) {
+    const double el = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - s.clock0).count();
+    if (el > s.timeout_ms && is_converged(s.p, s.delta, 10.0)) { s.converged = 1; lm_finish(s); return; }
+    else if (el > 1.5 * s.timeout_ms) { lm_finish(s); return; }
+  }
+  if (s.stationary && !s.converged) {
+    // A stationary point of the reference's loop: the FIRST LM trial was rejected (rho < 0) yet small enough for
+    // is_converged_low, so step_lm returned with x0 and lambda untouched (lsq_registration_impl.hpp:190-193) — and
+    // the step is not small enough for is_converged.  The next iteration linearises at the same x0 with the same lambda:
+    // with deterministic sums it is this iteration again, and again, to the iteration cap (measured on config 3: 60 of
+    // 64 iterations, the same 1.05 cm / 0.001 deg step each; the reference's CUDA build leaves it through the run-to-run
+    // noise of its fp32 atomic sums).  The outcome is known without running them: without a time budget the loop ends at
+    // the cap unconverged; with one it ends when the budget is spent, converged by is_converged_low (:94-104).
+    if (s.timeout_ms > 0) s.converged = 1;
+    else s.iterations = s.p.max_iterations - 1;
+    lm_finish(s);
+    return;
+  }
+  s.it++;
+  if (s.it >= s.p.max_iterations || s.converged) { lm_finish(s); return; }
+  s.iterations = s.it;
+  memcpy(s.want_T, s.x0, sizeof(s.x0));
+  s.want_update = true;
+}
+
+static void lm_begin(LmState& s, const lsd_reg_params_t& p, const double* guess) {
+  s.p = p;
+  memcpy(s.x0, guess, sizeof(s.x0));
+  s.lambda = -1.0;
+  s.converged = 0;
+  s.iterations = 0;
+  s.it = 0;
+  s.done = false;
+  s.h_set = false;
+  s.clock0 = std::chrono::steady_clock::now();
+  s.timeout_ms = (double)(p.max_process_time_us / 1000);
+  s.iter_log.clear();
+  if (p.max_iterations <= 0) { lm_finish(s); return; }
+  memcpy(s.want_T, s.x0, sizeof(s.x0));
+  s.want_update = true;
+}
+
+// The result of the evaluation the state asked for: H/b/err of linearize(want_T), or err of compute_error(want_T).
+static void lm_feed(LmState& s, const double* H, const double* b, double err) {
+  if (s.want_update) {
+    memcpy(s.H, H, sizeof(s.H)); memcpy(s.b, b, sizeof(s.b)); s.y0 = err;
+    if (s.lambda < 0.0) { double m = 0; for (int i = 0; i < 6; i++) m = std::max(m, fabs(s.H[7 * i])); s.lambda = s.p.lm_init_lambda_factor * m; }
+    s.nu = 2.0;
+    s.stepped = false; s.stationary = false;
+    s.trial = 0;
+    lm_try_trial(s);
+    return;
+  }
+  const double yi = err;
+  double den = 0;
+  for (int k = 0; k < 6; k++) den += s.d[k] * (s.lambda * s.d[k] - s.b[k]);
+  const double rho = (s.y0 - yi) / den;
+  if (rho < 0) {
+    if (is_converged(s.p, s.delta, 10.0)) { s.stepped = true; s.stationary = (s.trial == 0); lm_end_outer(s); return; }
+    s.lambda = s.nu * s.lambda; s.nu = 2 * s.nu;
+    s.trial++;
+    lm_try_trial(s);
+    return;
+  }
+  memcpy(s.x0, s.xi, sizeof(s.xi));
+  s.lambda = s.lambda * std::max(1.0 / 3.0, 1 - pow(2 * rho - 1, 3));
+  memcpy(s.final_H, s.H, sizeof(s.H));
+  s.h_set = true;
+  s.stepped = true;
+  lm_end_outer(s);
+}
+
 static lsd_status_t reg_align(lsd_reg* r, const double* guess) {
-  double x0[16];
-  memcpy(x0, guess, sizeof(x0));
-  double lambda = -1.0;
+  LmState s;
+  lm_begin(s, r->p, guess);
   r->converged = 0;
   r->iterations = 0;
-  const auto clock0 = std::chrono::steady_clock::now();
-  const double timeout_ms = (double)(r->p.max_process_time_us / 1000);
   r->iter_log.clear();
-  for (int it = 0; it < r->p.max_iterations && !r->converged; it++) {
-    r->iterations = it;
-    double H[36], b[6], y0, delta[16];
-    lsd_status_t s = reg_cost(r, x0, true, H, b, &y0, nullptr);
-    if (s < 0) return s;
-    if (lambda < 0.0) { double m = 0; for (int i = 0; i < 6; i++) m = std::max(m, fabs(H[7 * i])); lambda = r->p.lm_init_lambda_factor * m; }
-    double nu = 2.0;
-    bool stepped = false, stationary = false;
-    for (int i = 0; i < r->p.lm_max_iterations; i++) {
-      double d[6], xi[16], yi;
-      if (!solve6(H, lambda, b, d)) break;
-      se3_exp(d, delta);
-      mat4_mul(delta, x0, xi);
-      s = reg_cost(r, xi, false, nullptr, nullptr, &yi, nullptr);
-      if (s < 0) return s;
-      double den = 0;
-      for (int k = 0; k < 6; k++) den += d[k] * (lambda * d[k] - b[k]);
-      const double rho = (y0 - yi) / den;
-      if (rho < 0) {
-        if (is_converged(r, delta, 10.0)) { stepped = true; stationary = (i == 0); break; }
-        lambda = nu * lambda; nu = 2 * nu;
-        continue;
-      }
-      memcpy(x0, xi, sizeof(xi));
-      lambda = lambda * std::max(1.0 / 3.0, 1 - pow(2 * rho - 1, 3));
-      memcpy(r->final_H, H, sizeof(H));
-      stepped = true;
-      break;
-    }
-    if (!stepped) break;  // "lm not converged!!"
-    r->converged = is_converged(r, delta, 1.0) ? 1 : 0;
-    {  // what is_converged looked at (lsd_reg_iteration_log): |t|_inf of the step, its rotation angle, the cost it started from
-      double tm = 0; for (int k = 0; k < 3; k++) tm = std::max(tm, fabs(delta[4 * k + 3]));
-      r->iter_log.push_back(tm); r->iter_log.push_back(rot_angle(delta) / M_PI * 180.0); r->iter_log.push_back(y0); r->iter_log.push_back(lambda);
-    }
-    if (timeout_ms > 0) {
-      const double el = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - clock0).count();
-      if (el > timeout_ms && is_converged(r, delta, 10.0)) { r->converged = 1; break; }
-      else if (el > 1.5 * timeout_ms) break;
-    }
-    if (stationary && !r->converged) {
-      // A stationary point of the reference's loop: the FIRST LM trial was rejected (rho < 0) yet small enough for
-      // is_converged_low, so step_lm returned with x0 and lambda untouched (lsq_registration_impl.hpp:190-193) — and
-      // the step is not small enough for is_converged.  The next iteration linearises at the same x0 with the same lambda:
-      // with deterministic sums it is this iteration again, and again, to the iteration cap (measured on config 3: 60 of
-      // 64 iterations, the same 1.05 cm / 0.001 deg step each; the reference's CUDA build leaves it through the run-to-run
-      // noise of its fp32 atomic sums).  The outcome is known without running them: without a time budget the loop ends at
-      // the cap unconverged; with one it ends when the budget is spent, converged by is_converged_low (:94-104).
-      if (timeout_ms > 0) r->converged = 1;
-      else r->iterations = r->p.max_iterations - 1;
-      break;
-    }
+  while (!s.done) {
+    double H[36], b[6], y;
+    lsd_status_t st = reg_cost(r, s.want_T, s.want_update, s.want_update ? H : nullptr, b, &y, nullptr);
+    if (st < 0) return st;
+    lm_feed(s, H, b, y);
+    r->iterations = s.iterations;
   }
-  memcpy(r->final_T, x0, sizeof(x0));
+  r->converged = s.converged;
+  r->iterations = s.iterations;
+  r->iter_log.swap(s.iter_log);
+  if (s.h_set) memcpy(r->final_H, s.final_H, sizeof(s.final_H));
+  memcpy(r->final_T, s.x0, sizeof(s.x0));
   return LSD_OK;
 }
 

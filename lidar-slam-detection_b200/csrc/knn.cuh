@@ -37,6 +37,16 @@ struct WarpList {
 };
 constexpr int kWarpListBytes = kCandCap * 12;
 
+// the empty list of warp `warp` in a block's s_list[warps * kWarpListBytes]
+__device__ __forceinline__ WarpList make_warp_list(unsigned char* s_list, int warp) {
+  WarpList wl;
+  wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
+  wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
+  wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
+  wl.n = 0;
+  return wl;
+}
+
 #ifdef LSD_SIMT_EMU  // tests/simt: the host emulator has no PTX
 __device__ __forceinline__ unsigned lanemask_lt() { return simt_lanemask_lt(); }
 #else

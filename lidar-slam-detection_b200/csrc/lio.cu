@@ -548,11 +548,7 @@ __global__ void __launch_bounds__(kHmWarps * 32, 4) lio_knn_kernel(MapView mv, i
       }
     if (blockIdx.x == 0 && threadIdx.x == 0) rows[resize_parity] = n >= 5 ? n : prev;
   }
-  WarpList wl;
-  wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
-  wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
-  wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
-  wl.n = 0;
+  WarpList wl = make_warp_list(s_list, warp);
   wl.cell = ref_order ? s_cell[warp] : nullptr;
   const LaneStencil ls = lane_stencil(stencil_slot(stencil));
   // (An L2-prefetch pass over the warp's queries was measured here and removed: +9 us per launch —
@@ -998,24 +994,27 @@ struct ProfScope {  // CUDA-event timing of one launch group on the LIO stream (
   }
 };
 
-// Spin on the sequence number the kernel publishes into mapped host memory.  The load is an acquire: the sums the
+// Spin on the sequence number a kernel publishes into mapped host memory at `slot`.  The load is an acquire: the sums the
 // kernel stored before the sequence number must not be read ahead of it (aarch64 hosts reorder loads).  Bounded by a
 // wall-clock limit so that a hung kernel (e.g. a peer that never answers the in-kernel all-reduce) becomes an error.
-static lsd_status_t wait_seq(lsd_lio* l, int slot, double seq) {
-  const double* r = l->h_result + slot;
+// Used by the LIO front end, the matcher (reg.cu) and the loop detector (loop.cu).
+static lsd_status_t wait_seq(const double* slot, cudaStream_t stream, double seq, double timeout_s) {
+  const unsigned long long* h = reinterpret_cast<const unsigned long long*>(slot);
+  unsigned long long want;
+  memcpy(&want, &seq, 8);
   const auto t0 = std::chrono::steady_clock::now();
   for (unsigned long long spins = 0;; spins++) {
-    if (__atomic_load_n(reinterpret_cast<const unsigned long long*>(r), __ATOMIC_ACQUIRE) == *reinterpret_cast<const unsigned long long*>(&seq)) return LSD_OK;
+    if (__atomic_load_n(h, __ATOMIC_ACQUIRE) == want) return LSD_OK;
     if ((spins & 0xfff) == 0xfff) {
-      cudaError_t e = cudaStreamQuery(l->stream);
+      cudaError_t e = cudaStreamQuery(stream);
       if (e != cudaSuccess && e != cudaErrorNotReady) return cuda_fail(e, "kernel while waiting for the reduction", __FILE__, __LINE__);
       if (e == cudaSuccess) {  // stream drained: the result must be there
-        if (__atomic_load_n(reinterpret_cast<const unsigned long long*>(r), __ATOMIC_ACQUIRE) == *reinterpret_cast<const unsigned long long*>(&seq)) return LSD_OK;
+        if (__atomic_load_n(h, __ATOMIC_ACQUIRE) == want) return LSD_OK;
         set_error("reduction result never published");
         return LSD_ERR_CUDA;
       }
-      if (std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > l->wait_timeout_s) {
-        set_error("timed out after %.0f s waiting for a reduction result (kernel hung?)", l->wait_timeout_s);
+      if (std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > timeout_s) {
+        set_error("timed out after %.0f s waiting for a reduction result (kernel hung?)", timeout_s);
         return LSD_ERR_CUDA;
       }
     }
@@ -1071,7 +1070,7 @@ lsd_status_t lio_linearize(lsd_lio* l, const double* x, bool search, double* HTH
   LSD_CUDA(cudaGetLastError());
   prof.stop();
   if (l->issue_in_linearize) { lsd_status_t d = issue_deferred_prefetch(l); if (d) return d; }   // hidden under this evaluation
-  { lsd_status_t w = wait_seq(l, kResSeq, seq); if (w) return w; }
+  { lsd_status_t w = wait_seq(l->h_result + kResSeq, l->stream, seq, l->wait_timeout_s); if (w) return w; }
   const double* r = l->h_result;
   if (l->sc.world > 1) { l->xchg_cycles += r[kResWaitCycles]; l->xchg_count++; }
   int q = 0;
@@ -1101,7 +1100,7 @@ lsd_status_t lio_linearize(lsd_lio* l, const double* x, bool search, double* HTH
                  l->d_done, l->d_result, seq, l->sc);
       LSD_CUDA(cudaGetLastError());
       l->launches++;
-      { lsd_status_t w = wait_seq(l, kResSeqDegen, seq); if (w) return w; }
+      { lsd_status_t w = wait_seq(l->h_result + kResSeqDegen, l->stream, seq, l->wait_timeout_s); if (w) return w; }
       const double* dg = l->h_result + kResDegen;
       int mask[3] = {1, 1, 1};
       bool deg = false;

@@ -5,9 +5,10 @@
 // cost evaluation, one host round trip.  Here every candidate keeps its own LM state (LmState, reg.cu) and the states
 // advance together: one ndt_cost_batch_kernel launch per round evaluates the next cost of every live candidate against
 // the new key frame's NDT map, so a detect costs as many round trips as its slowest candidate, not their sum.
-// Per candidate the launch is the single-pair launch: reg_grid(n_c) blocks with the same point-to-block partition
-// (ndt_point, reg.cu), the same block_partials<29> and the same last-block fold over those blocks — H, b, err and the
-// correspondence count are the bits of ndt_cost_kernel, so the LM trajectory is that of a separate lsd_reg handle.
+// Per candidate the launch is the single-pair launch: reg_grid(n_c) blocks with the same point-to-block partition, the
+// per-point body ndt_cost_kernel runs (ndt_point, reg.cu), the same block_partials<29> and a last-block fold over those
+// blocks in grid_finalize's order — H, b, err and the correspondence count are the bits of ndt_cost_kernel, so the LM
+// trajectory is that of a separate lsd_reg handle.  The fitness launch runs lsd_reg_fitness's body (fitness_range).
 // Included by lsdreg.cu after reg.cu (uses its kernels' building blocks and the host helpers).
 
 namespace lsd {
@@ -19,7 +20,7 @@ struct LoopCand {
   long long corr_off;    // NDT: [n_off, n] correspondence slots at this offset of the correspondence pool
   int row;               // result row (candidate index in the caller's list)
   int update, deriv;     // NDT: linearize (refresh correspondences) / accumulate H and b
-  int warp_shape;        // fitness: one warp per point (fitness_kernel) instead of one thread (fitness_thread_kernel)
+  int warp_shape;        // fitness: fitness_range<true> (one warp per point) instead of <false> (one thread), as lsd_reg_fitness
   Pose34f lin, ev;       // NDT: linearisation / evaluation pose; fitness: ev is the pose
 };
 
@@ -102,77 +103,22 @@ __global__ void __launch_bounds__(256) ndt_cost_batch_kernel(NdtView v, const fl
                     result + (size_t)(1 + cands[c].row) * kNV, result, seq);
 }
 
-// Exact nearest-neighbour distance by a scan of the whole target, for points with nothing inside the grid search radius:
-// calc_fitness_score counts every point however far (max_range = DBL_MAX).  Thread version.
-__device__ __forceinline__ float nn_scan_thread(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz) {
-  float bd = 3.0e38f;
-  for (int j = 0; j < n_tgt; j++) { const float4 b = __ldg(tgt + j); bd = fminf(bd, dist2(qx, qy, qz, b.x, b.y, b.z)); }
-  return bd;
-}
-// Warp version: lanes stride over the target, then a min across lanes (every lane returns it).
-__device__ __forceinline__ float nn_scan_warp(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz) {
-  float bd = 3.0e38f;
-  for (int j = threadIdx.x & 31; j < n_tgt; j += 32) { const float4 b = __ldg(tgt + j); bd = fminf(bd, dist2(qx, qy, qz, b.x, b.y, b.z)); }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) bd = fminf(bd, __shfl_xor_sync(0xffffffffu, bd, o));
-  return bd;
-}
-
 // getFitnessScore(max_range) of every candidate at its pose against the new key frame's point map.  Per candidate the
-// shape, grid and fold of lsd_reg_fitness (fitness_kernel / fitness_thread_kernel, reg.cu): same sum, same count.
-// tgt != nullptr: points with no neighbour within search_sq get the exact one (nn_scan_*), for calc_fitness_score.
+// shape and grid of lsd_reg_fitness and the same body (fitness_range, reg.cu) and fold: same sum, same count.
+// tgt != nullptr: points with no neighbour within search_sq get the exact one, for calc_fitness_score.
 __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_batch_kernel(MapView mv, const float4* __restrict__ pool,
                                                                           const LoopCand* __restrict__ cands, int n_cand, float search_sq,
                                                                           float max_range, const float4* __restrict__ tgt, int n_tgt,
                                                                           double* __restrict__ partials, unsigned* __restrict__ done,
                                                                           double* __restrict__ result, double seq) {
-  __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
-  __shared__ double s_acc[kRegWarps][2];
   const int c = loop_cand_of_block(cands, n_cand);
   const int n = cands[c].n, G = cands[c].n_blk, lb = (int)blockIdx.x - cands[c].blk_off;
   const Pose34f Tf = cands[c].ev;
   const float4* src = pool + cands[c].src_off;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  double sum = 0.0, cnt = 0.0;
-  if (cands[c].warp_shape) {  // block-uniform
-    WarpList wl;
-    wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
-    wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
-    wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
-    wl.n = 0;
-    for (int i = lb * kRegWarps + warp; i < n; i += G * kRegWarps) {
-      const float4 a = __ldg(src + i);
-      const float qx = Tf.R[0] * a.x + Tf.R[1] * a.y + Tf.R[2] * a.z + Tf.t[0];
-      const float qy = Tf.R[3] * a.x + Tf.R[4] * a.y + Tf.R[5] * a.z + Tf.t[1];
-      const float qz = Tf.R[6] * a.x + Tf.R[7] * a.y + Tf.R[8] * a.z + Tf.t[2];
-      Neighbor nb;
-      const int nf = knn_exact_warp<1>(mv, qx, qy, qz, search_sq, wl, nb);
-      float d2 = __shfl_sync(kFull, nb.d2, 0);
-      bool found = nf > 0;
-      if (!found && tgt) { d2 = nn_scan_warp(tgt, n_tgt, qx, qy, qz); found = n_tgt > 0; }   // warp-uniform
-      if (found && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
-    }
-    if (lane == 0) { s_acc[warp][0] = sum; s_acc[warp][1] = cnt; }
-  } else {
-    for (int i = lb * blockDim.x + threadIdx.x; i < n; i += G * blockDim.x) {
-      const float4 a = __ldg(src + i);
-      const float qx = Tf.R[0] * a.x + Tf.R[1] * a.y + Tf.R[2] * a.z + Tf.t[0];
-      const float qy = Tf.R[3] * a.x + Tf.R[4] * a.y + Tf.R[5] * a.z + Tf.t[1];
-      const float qz = Tf.R[6] * a.x + Tf.R[7] * a.y + Tf.R[8] * a.z + Tf.t[2];
-      float d2; int id;
-      bool found = nn1_exact_thread(mv, qx, qy, qz, search_sq, &d2, &id);
-      if (!found && tgt) { d2 = nn_scan_thread(tgt, n_tgt, qx, qy, qz); found = n_tgt > 0; }
-      if (found && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
-    }
-    sum = warp_sum(sum); cnt = warp_sum(cnt);
-    if (lane == 0) { s_acc[warp][0] = sum; s_acc[warp][1] = cnt; }
-  }
-  __syncthreads();
-  if (threadIdx.x < 2) {
-    double s = 0.0;
-    for (int w = 0; w < kRegWarps; w++) s += s_acc[w][threadIdx.x];
-    partials[(size_t)blockIdx.x * kNV + threadIdx.x] = s;
-  }
+  if (cands[c].warp_shape)  // block-uniform
+    fitness_range<true>(mv, src, n, lb, G, Tf, search_sq, max_range, tgt, n_tgt, partials);
+  else
+    fitness_range<false>(mv, src, n, lb, G, Tf, search_sq, max_range, tgt, n_tgt, partials);
   loop_finalize<2>(partials + (size_t)cands[c].blk_off * kNV, G, done + 1 + c, done, n_cand,
                    result + (size_t)(1 + cands[c].row) * kNV, result, seq);
 }
@@ -277,16 +223,16 @@ static lsd_status_t loop_fitness(lsd_loop* h, const std::vector<int>& slots, con
   cudaStream_t st = r->stream;
   LSD_CUDA(cudaMemcpyAsync(h->d_cand, h->h_cand, n * sizeof(LoopCand), cudaMemcpyHostToDevice, st));
   const double seq = (double)(++h->seq);
-  const float search_sq = (float)std::min(max_range, 64.0 * r->p.map_resolution * r->p.map_resolution * 64.0);
+  const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
   fitness_batch_kernel<<<blocks, kRegWarps * 32, 0, st>>>(r->tgt_map->view, h->d_pool, h->d_cand, n, search_sq, (float)max_range,
                                                          exact ? r->d_tgt : nullptr, r->n_tgt, h->d_partials, h->d_done, h->d_res, seq);
   LSD_CUDA(cudaGetLastError());
   (*launches)++;
-  s = wait_seq(h->h_res, st, seq);
+  s = wait_seq(h->h_res, st, seq, 20.0);
   if (s) return s;
   for (int i = 0; i < n; i++) {
     const double sum = h->h_res[(size_t)(1 + i) * kNV], cnt = h->h_res[(size_t)(1 + i) * kNV + 1];
-    score[i] = cnt > 0 ? sum / cnt : 1.7976931348623157e308;
+    score[i] = cnt > 0 ? sum / cnt : DBL_MAX;
     if (count) count[i] = cnt;
   }
   return LSD_OK;
@@ -330,18 +276,14 @@ static lsd_status_t loop_coarse(lsd_loop* h, int target, const int32_t* cand, co
     ndt_cost_batch_kernel<<<blocks, 256, 0, st>>>(r->ndt, h->d_pool, h->d_cand, na, n_off, h->d_corr, h->d_partials, h->d_done, h->d_res, seq);
     LSD_CUDA(cudaGetLastError());
     (*launches)++; (*rounds)++;
-    s = wait_seq(h->h_res, st, seq);
+    s = wait_seq(h->h_res, st, seq, 20.0);
     if (s) return s;
     for (int i = 0; i < n; i++) {
       LmState& m = h->lm[i];
       if (m.done) continue;
       const double* res = h->h_res + (size_t)(1 + i) * kNV;
       double H[36], b[6];
-      if (m.want_update) {
-        int q = 0;
-        for (int a = 0; a < 6; a++) for (int c = a; c < 6; c++) { H[6 * a + c] = H[6 * c + a] = res[q]; q++; }
-        for (int a = 0; a < 6; a++) b[a] = res[21 + a];
-      }
+      if (m.want_update) unpack_hb(res, H, b);
       lm_feed(m, H, b, res[27]);
     }
   }
@@ -606,7 +548,7 @@ lsd_status_t lsd_loop_detect(lsd_loop_t* h, const double* poses16, const int32_t
   std::vector<double> guesses;
   for (int q = 0; q < n_new; q++) {
     const int32_t ns = new_keyframes[q];
-    lsd_loop_report_t rep = {ns, LSD_LOOP_SKIPPED, 0, -1, 1.7976931348623157e308};
+    lsd_loop_report_t rep = {ns, LSD_LOOP_SKIPPED, 0, -1, DBL_MAX};
     if (accum[ns] - acc_new < h->p.distance_new_keyframe_thresh) { h->reports.push_back(rep); continue; }
     acc_new = accum[ns];
     const int nc = loop_find(h->p, h->last_edge, poses16, accum, keyframes, n_kf, ns, cand);
@@ -619,7 +561,7 @@ lsd_status_t lsd_loop_detect(lsd_loop_t* h, const double* poses16, const int32_t
     if (s) return s;
     // best candidate (:175-191): converged only; a later candidate with an equal score wins
     int best = -1;
-    double best_score = 1.7976931348623157e308;
+    double best_score = DBL_MAX;
     for (int i = 0; i < nc; i++) {
       if (!h->lm[i].converged) continue;
       if (h->fitness[i] > best_score) continue;
@@ -653,7 +595,7 @@ lsd_status_t lsd_loop_detect(lsd_loop_t* h, const double* poses16, const int32_t
     res.coarse_score = best_score; res.score = score; res.n_candidates = nc;
     // calc_information_matrix(key1->cloud, key2->cloud, relpose): calc_fitness_score with max_range = DBL_MAX
     double fit = 0;
-    s = lsd_loop_fitness(h, ns, cand[best], res.relpose16, 1.7976931348623157e308, &fit, nullptr);
+    s = lsd_loop_fitness(h, ns, cand[best], res.relpose16, DBL_MAX, &fit, nullptr);
     if (s) return s;
     loop_information(fit, res.information36);
     if (*n_loops < cap) out[*n_loops] = res;

@@ -153,11 +153,7 @@ __global__ void __launch_bounds__(kKnnWarps * 32, 5) knn_query_kernel(MapView mv
                                                                    float* __restrict__ out_d2, int* __restrict__ out_cnt) {
   __shared__ __align__(16) unsigned char s_list[kKnnWarps * kWarpListBytes];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  WarpList wl;
-  wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
-  wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
-  wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
-  wl.n = 0;
+  WarpList wl = make_warp_list(s_list, warp);
   const LaneStencil ls = lane_stencil(stencil_slot(stencil));
   for (int i = blockIdx.x * kKnnWarps + warp; i < nq; i += gridDim.x * kKnnWarps) {
     const float4 p = __ldg(q + i);

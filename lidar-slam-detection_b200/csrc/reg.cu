@@ -20,7 +20,9 @@
 //   * GICP neighbours come from the hash-voxel map's exact search (knn.cuh) instead of a k-d tree.
 #include <unistd.h>
 
+#include <cfloat>
 #include <chrono>
+#include <type_traits>
 #include <vector>
 
 #include "knn.cuh"
@@ -41,6 +43,20 @@ __device__ __forceinline__ int3 ndt_coord(float x, float y, float z, float res) 
   return make_int3((int)floorf(x / res - 0.5f), (int)floorf(y / res - 0.5f), (int)floorf(z / res - 0.5f));
 }
 
+// The build-table slot of voxel `key` (open addressing, linear probing), claimed if the voxel is new; -1 when kMaxProbe
+// probes find neither the key nor a free slot.  Both voxel maps (NDT, VGICP) are accumulated through here.
+__device__ __forceinline__ long long claim_slot(NdtBuildLine* __restrict__ tab, unsigned long long mask, unsigned long long key) {
+  unsigned long long s = hash_key(key) & mask;
+  for (unsigned probe = 0; probe < kMaxProbe; probe++) {
+    unsigned long long* kp = &tab[s].key;
+    unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(kp);
+    if (cur == 0ull) cur = atomicCAS(kp, 0ull, key), cur = cur == 0ull ? key : cur;
+    if (cur == key) return (long long)s;
+    s = (s + 1) & mask;
+  }
+  return -1;
+}
+
 // Tile-sharded target (SURVEY.md section 8e, row C3): with world > 1 a rank keeps only the voxels of the x-y tiles it owns
 // (tile_owner, lsd_common.cuh).  Every (source point, stencil offset) pair then finds its voxel on exactly one rank, so the
 // ranks' sums partition the single-GPU sums and the in-kernel all-reduce (grid_finalize) restores them: no halo needed.
@@ -53,23 +69,13 @@ __global__ void __launch_bounds__(256) ndt_accum_kernel(NdtBuildLine* __restrict
   const int3 c = ndt_coord(p.x, p.y, p.z, res);
   if (!coord_ok(c.x, c.y, c.z)) { atomicAdd(fail, 1u); return; }
   if (shard_world > 1 && tile_owner(c.x, c.y, shard_tile, shard_world) != shard_rank) return;   // another rank's voxel
-  const unsigned long long key = pack_key(c.x, c.y, c.z, 0);
-  unsigned long long s = hash_key(key) & mask;
-  for (unsigned probe = 0; probe < kMaxProbe; probe++) {
-    unsigned long long* kp = &tab[s].key;
-    unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(kp);
-    if (cur == 0ull) cur = atomicCAS(kp, 0ull, key), cur = cur == 0ull ? key : cur;
-    if (cur == key) {
-      atomicAdd(&tab[s].count, 1u);
-      const double x = p.x, y = p.y, z = p.z;
-      atomicAdd(&tab[s].sum[0], x); atomicAdd(&tab[s].sum[1], y); atomicAdd(&tab[s].sum[2], z);
-      atomicAdd(&tab[s].sxx[0], x * x); atomicAdd(&tab[s].sxx[1], x * y); atomicAdd(&tab[s].sxx[2], x * z);
-      atomicAdd(&tab[s].sxx[3], y * y); atomicAdd(&tab[s].sxx[4], y * z); atomicAdd(&tab[s].sxx[5], z * z);
-      return;
-    }
-    s = (s + 1) & mask;
-  }
-  atomicAdd(fail, 1u);
+  const long long s = claim_slot(tab, mask, pack_key(c.x, c.y, c.z, 0));
+  if (s < 0) { atomicAdd(fail, 1u); return; }
+  atomicAdd(&tab[s].count, 1u);
+  const double x = p.x, y = p.y, z = p.z;
+  atomicAdd(&tab[s].sum[0], x); atomicAdd(&tab[s].sum[1], y); atomicAdd(&tab[s].sum[2], z);
+  atomicAdd(&tab[s].sxx[0], x * x); atomicAdd(&tab[s].sxx[1], x * y); atomicAdd(&tab[s].sxx[2], x * z);
+  atomicAdd(&tab[s].sxx[3], y * y); atomicAdd(&tab[s].sxx[4], y * z); atomicAdd(&tab[s].sxx[5], z * z);
 }
 
 // smallest-eigenvalue direction of a symmetric 3x3 (double, cyclic Jacobi)
@@ -121,7 +127,9 @@ __global__ void __launch_bounds__(256) ndt_finalize_kernel(const NdtBuildLine* _
   out[s] = o;
 }
 
-__device__ __forceinline__ int ndt_lookup(const NdtView& v, int x, int y, int z) {
+// Slot of voxel (x, y, z) in a finalised voxel table (NdtView, VgView), -1 if absent.
+template <class View>
+__device__ __forceinline__ int voxel_lookup(const View& v, int x, int y, int z) {
   if (!coord_ok(x, y, z)) return -1;
   const unsigned long long key = pack_key(x, y, z, 0);
   unsigned long long s = hash_key(key) & v.mask;
@@ -134,8 +142,26 @@ __device__ __forceinline__ int ndt_lookup(const NdtView& v, int x, int y, int z)
   return -1;
 }
 
-struct Pose34f { float R[9], t[3]; };
+// Offset o of the DIRECT1 / DIRECT7 / DIRECT27 neighbour stencil (n_off = 1, 7, 27)
 __constant__ signed char c_ndt_off7[7][3] = {{0,0,0},{1,0,0},{-1,0,0},{0,1,0},{0,-1,0},{0,0,1},{0,0,-1}};
+__device__ __forceinline__ int3 stencil_offset(int o, int n_off) {
+  if (n_off == 27) return make_int3(o / 9 - 1, (o / 3) % 3 - 1, o % 3 - 1);
+  return make_int3(c_ndt_off7[o][0], c_ndt_off7[o][1], c_ndt_off7[o][2]);
+}
+
+struct Pose34f { float R[9], t[3]; };
+struct Pose34d { double R[9], t[3]; };
+
+// R a + t
+__device__ __forceinline__ float3 xform(const Pose34f& T, const float4 a) {
+  return make_float3(T.R[0] * a.x + T.R[1] * a.y + T.R[2] * a.z + T.t[0], T.R[3] * a.x + T.R[4] * a.y + T.R[5] * a.z + T.t[1],
+                     T.R[6] * a.x + T.R[7] * a.y + T.R[8] * a.z + T.t[2]);
+}
+__device__ __forceinline__ double3 xform(const Pose34d& T, const float4 a) {
+  const double ax = a.x, ay = a.y, az = a.z;
+  return make_double3(T.R[0] * ax + T.R[1] * ay + T.R[2] * az + T.t[0], T.R[3] * ax + T.R[4] * ay + T.R[5] * az + T.t[1],
+                      T.R[6] * ax + T.R[7] * ay + T.R[8] * az + T.t[2]);
+}
 
 // One source point of an NDT cost evaluation (find_voxel_correspondences + p2d_ndt_compute_derivatives).  `corr` points at
 // the [n_off, n] correspondence slots of this cloud.  Shared by the single-pair kernel below (compile-time flags) and the
@@ -143,24 +169,19 @@ __constant__ signed char c_ndt_off7[7][3] = {{0,0,0},{1,0,0},{-1,0,0},{0,1,0},{0
 __device__ __forceinline__ void ndt_point(const NdtView& v, const float4 a, int i, int n, int n_off, const Pose34f& lin,
                                           const Pose34f& ev, int* __restrict__ corr, bool update, bool deriv, double (&vals)[29]) {
   const float k_sq = v.res * v.res;
-  const float tx = ev.R[0] * a.x + ev.R[1] * a.y + ev.R[2] * a.z + ev.t[0];
-  const float ty = ev.R[3] * a.x + ev.R[4] * a.y + ev.R[5] * a.z + ev.t[1];
-  const float tz = ev.R[6] * a.x + ev.R[7] * a.y + ev.R[8] * a.z + ev.t[2];
+  const float3 t = xform(ev, a);
+  const float tx = t.x, ty = t.y, tz = t.z;
   int3 c = make_int3(0, 0, 0);
   if (update) {
-    const float lx = lin.R[0] * a.x + lin.R[1] * a.y + lin.R[2] * a.z + lin.t[0];
-    const float ly = lin.R[3] * a.x + lin.R[4] * a.y + lin.R[5] * a.z + lin.t[1];
-    const float lz = lin.R[6] * a.x + lin.R[7] * a.y + lin.R[8] * a.z + lin.t[2];
-    c = ndt_coord(lx, ly, lz, v.res);
+    const float3 l = xform(lin, a);
+    c = ndt_coord(l.x, l.y, l.z, v.res);
   }
 #pragma unroll 1
   for (int o = 0; o < n_off; o++) {
     int slot;
     if (update) {
-      int ox, oy, oz;
-      if (n_off == 27) { ox = o / 9 - 1; oy = (o / 3) % 3 - 1; oz = o % 3 - 1; }
-      else { ox = c_ndt_off7[o][0]; oy = c_ndt_off7[o][1]; oz = c_ndt_off7[o][2]; }
-      slot = ndt_lookup(v, c.x + ox, c.y + oy, c.z + oz);
+      const int3 d = stencil_offset(o, n_off);
+      slot = voxel_lookup(v, c.x + d.x, c.y + d.y, c.z + d.z);
       corr[(size_t)o * n + i] = slot;
     } else {
       slot = corr[(size_t)o * n + i];
@@ -220,35 +241,39 @@ __global__ void __launch_bounds__(256) ndt_cost_kernel(NdtView v, const float4* 
 // k-NN covariance -> smallest-eigenvalue direction (calculate_covariances, fast_gicp_impl.hpp:244-303).
 // One warp per point: exact K-NN, lanes hold the neighbours, warp-shuffle moments in double.
 constexpr int kRegWarps = 8;
+
+// Lanes 0 .. k-1 hold the k neighbours (x, y, z; zero in lanes without one): the k-column mean and covariance, its
+// smallest-eigenvalue direction, stored by lane 0 with nf, the neighbour count, into nrm[4 i .. 4 i + 4).
+__device__ __forceinline__ void warp_normal(double x, double y, double z, int k, int nf, double* __restrict__ nrm, int i) {
+  const int lane = threadIdx.x & 31;
+  const double kk = (double)k;
+  const double mx = warp_sum(x) / kk, my = warp_sum(y) / kk, mz = warp_sum(z) / kk;   // rowwise().mean() over k columns
+  const double dx = (lane < k ? x : 0.0) - (lane < k ? mx : 0.0), dy = (lane < k ? y : 0.0) - (lane < k ? my : 0.0),
+               dz = (lane < k ? z : 0.0) - (lane < k ? mz : 0.0);
+  double C[9];
+  C[0] = warp_sum(dx * dx) / kk; C[1] = warp_sum(dx * dy) / kk; C[2] = warp_sum(dx * dz) / kk;
+  C[4] = warp_sum(dy * dy) / kk; C[5] = warp_sum(dy * dz) / kk; C[8] = warp_sum(dz * dz) / kk;
+  C[3] = C[1]; C[6] = C[2]; C[7] = C[5];
+  if (lane == 0) {
+    double nr[3];
+    smallest_eigvec(C, nr);
+    double* o = nrm + 4 * (size_t)i;  // double: C = I - 0.999 n n^T is inverted with condition number 1000
+    o[0] = nr[0]; o[1] = nr[1]; o[2] = nr[2]; o[3] = (double)nf;
+  }
+}
+
 __global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_normals_kernel(MapView mv, const float4* __restrict__ pts, int n, int k,
                                                                          float max_sq, double* __restrict__ nrm) {
   __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  WarpList wl;
-  wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
-  wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
-  wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
-  wl.n = 0;
+  WarpList wl = make_warp_list(s_list, warp);
   for (int i = blockIdx.x * kRegWarps + warp; i < n; i += gridDim.x * kRegWarps) {
     const float4 p = __ldg(pts + i);
     Neighbor nb;
     const int nf = knn_exact_warp<20>(mv, p.x, p.y, p.z, max_sq, wl, nb);
     double x = 0, y = 0, z = 0;
     if (lane < min(nf, k)) { const float4 q = load_loc(mv, nb.loc); x = q.x; y = q.y; z = q.z; }
-    const double kk = (double)k;
-    const double mx = warp_sum(x) / kk, my = warp_sum(y) / kk, mz = warp_sum(z) / kk;   // rowwise().mean() over k columns
-    const double dx = (lane < k ? x : 0.0) - (lane < k ? mx : 0.0), dy = (lane < k ? y : 0.0) - (lane < k ? my : 0.0),
-                 dz = (lane < k ? z : 0.0) - (lane < k ? mz : 0.0);
-    double C[9];
-    C[0] = warp_sum(dx * dx) / kk; C[1] = warp_sum(dx * dy) / kk; C[2] = warp_sum(dx * dz) / kk;
-    C[4] = warp_sum(dy * dy) / kk; C[5] = warp_sum(dy * dz) / kk; C[8] = warp_sum(dz * dz) / kk;
-    C[3] = C[1]; C[6] = C[2]; C[7] = C[5];
-    if (lane == 0) {
-      double nr[3];
-      smallest_eigvec(C, nr);
-      double* o = nrm + 4 * (size_t)i;  // double: C = I - 0.999 n n^T is inverted with condition number 1000
-      o[0] = nr[0]; o[1] = nr[1]; o[2] = nr[2]; o[3] = (double)nf;
-    }
+    warp_normal(x, y, z, k, nf, nrm, i);
   }
 }
 
@@ -286,20 +311,7 @@ __global__ void __launch_bounds__(kRegWarps * 32) gicp_normals_complete_kernel(c
     const int nf = min(n, k);
     double x = 0, y = 0, z = 0;
     if (lane < nf) { const float4 q = __ldg(pts + bi); x = q.x; y = q.y; z = q.z; }
-    const double kk = (double)k;
-    const double mx = warp_sum(x) / kk, my = warp_sum(y) / kk, mz = warp_sum(z) / kk;
-    const double dx = (lane < k ? x : 0.0) - (lane < k ? mx : 0.0), dy = (lane < k ? y : 0.0) - (lane < k ? my : 0.0),
-                 dz = (lane < k ? z : 0.0) - (lane < k ? mz : 0.0);
-    double C[9];
-    C[0] = warp_sum(dx * dx) / kk; C[1] = warp_sum(dx * dy) / kk; C[2] = warp_sum(dx * dz) / kk;
-    C[4] = warp_sum(dy * dy) / kk; C[5] = warp_sum(dy * dz) / kk; C[8] = warp_sum(dz * dz) / kk;
-    C[3] = C[1]; C[6] = C[2]; C[7] = C[5];
-    if (lane == 0) {
-      double nr[3];
-      smallest_eigvec(C, nr);
-      double* o = nrm + 4 * (size_t)i;
-      o[0] = nr[0]; o[1] = nr[1]; o[2] = nr[2]; o[3] = (double)nf;
-    }
+    warp_normal(x, y, z, k, nf, nrm, i);
   }
 }
 
@@ -355,67 +367,10 @@ __device__ __forceinline__ bool nn1_exact_thread(const MapView& mv, float qx, fl
   return found;
 }
 
-struct Pose34d { double R[9], t[3]; };
-
-// update_correspondences (fast_gicp_impl.hpp:119-157): 1-NN of the transformed source point, Mahalanobis
-// matrix (C_B + R C_A R^T)^-1 in double.  One warp per source point.
-__global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv, const float4* __restrict__ src,
-                                                                      const double* __restrict__ src_nrm, int n,
-                                                                      const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
-                                                                      float max_corr_sq, int* __restrict__ corr,
-                                                                      double* __restrict__ maha) {
-  __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  WarpList wl;
-  wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
-  wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
-  wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
-  wl.n = 0;
-  for (int i = blockIdx.x * kRegWarps + warp; i < n; i += gridDim.x * kRegWarps) {
-    const float4 a = __ldg(src + i);
-    const float qx = Tf.R[0] * a.x + Tf.R[1] * a.y + Tf.R[2] * a.z + Tf.t[0];
-    const float qy = Tf.R[3] * a.x + Tf.R[4] * a.y + Tf.R[5] * a.z + Tf.t[1];
-    const float qz = Tf.R[6] * a.x + Tf.R[7] * a.y + Tf.R[8] * a.z + Tf.t[2];
-    Neighbor nb;
-    const int nf = knn_exact_warp<1>(mv, qx, qy, qz, max_corr_sq, wl, nb);
-    const float d2 = __shfl_sync(kFull, nb.d2, 0);
-    const int id = __shfl_sync(kFull, nb.id, 0);
-    if (lane != 0) continue;
-    const int c = (nf > 0 && d2 < max_corr_sq) ? id : -1;
-    corr[i] = c;
-    if (c < 0) continue;
-    const double* na = src_nrm + 4 * (size_t)i;
-    const double* nbv = tgt_nrm + 4 * (size_t)c;
-    const double rn[3] = {T.R[0] * na[0] + T.R[1] * na[1] + T.R[2] * na[2], T.R[3] * na[0] + T.R[4] * na[1] + T.R[5] * na[2],
-                          T.R[6] * na[0] + T.R[7] * na[1] + T.R[8] * na[2]};
-    double A[9];
-#pragma unroll
-    for (int p = 0; p < 3; p++)
-#pragma unroll
-      for (int q = 0; q < 3; q++) A[3 * p + q] = (p == q ? 2.0 : 0.0) - 0.999 * (nbv[p] * nbv[q] + rn[p] * rn[q]);
-    const double c00 = A[4] * A[8] - A[5] * A[7], c01 = A[5] * A[6] - A[3] * A[8], c02 = A[3] * A[7] - A[4] * A[6];
-    const double idet = 1.0 / (A[0] * c00 + A[1] * c01 + A[2] * c02);
-    double* M = maha + 6 * (size_t)i;  // symmetric: xx xy xz yy yz zz
-    M[0] = c00 * idet; M[1] = (A[2] * A[7] - A[1] * A[8]) * idet; M[2] = (A[1] * A[5] - A[2] * A[4]) * idet;
-    M[3] = (A[0] * A[8] - A[2] * A[6]) * idet; M[4] = (A[2] * A[3] - A[0] * A[5]) * idet; M[5] = (A[0] * A[4] - A[1] * A[3]) * idet;
-  }
-}
-
-// update_correspondences, batched shape: one thread per source point (nn1_exact_thread)
-__global__ void __launch_bounds__(256) gicp_corr_thread_kernel(MapView mv, const float4* __restrict__ src, const double* __restrict__ src_nrm,
-                                                               int n, const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
-                                                               float max_corr_sq, int* __restrict__ corr, double* __restrict__ maha) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float4 a = __ldg(src + i);
-  const float qx = Tf.R[0] * a.x + Tf.R[1] * a.y + Tf.R[2] * a.z + Tf.t[0];
-  const float qy = Tf.R[3] * a.x + Tf.R[4] * a.y + Tf.R[5] * a.z + Tf.t[1];
-  const float qz = Tf.R[6] * a.x + Tf.R[7] * a.y + Tf.R[8] * a.z + Tf.t[2];
-  float d2; int id;
-  const bool f = nn1_exact_thread(mv, qx, qy, qz, max_corr_sq, &d2, &id);
-  const int c = (f && d2 < max_corr_sq) ? id : -1;
-  corr[i] = c;
-  if (c < 0) return;
+// Mahalanobis matrix (C_B + R C_A R^T)^-1 of correspondence (source i, target c) at T, in double, stored symmetric
+// (xx xy xz yy yz zz) into maha[6 i ..].
+__device__ __forceinline__ void gicp_store_maha(const double* __restrict__ src_nrm, const double* __restrict__ tgt_nrm, int i, int c,
+                                                const Pose34d& T, double* __restrict__ maha) {
   const double* na = src_nrm + 4 * (size_t)i;
   const double* nbv = tgt_nrm + 4 * (size_t)c;
   const double rn[3] = {T.R[0] * na[0] + T.R[1] * na[1] + T.R[2] * na[2], T.R[3] * na[0] + T.R[4] * na[1] + T.R[5] * na[2],
@@ -432,6 +387,70 @@ __global__ void __launch_bounds__(256) gicp_corr_thread_kernel(MapView mv, const
   M[3] = (A[0] * A[8] - A[2] * A[6]) * idet; M[4] = (A[2] * A[3] - A[0] * A[5]) * idet; M[5] = (A[0] * A[4] - A[1] * A[3]) * idet;
 }
 
+// update_correspondences (fast_gicp_impl.hpp:119-157): 1-NN of the transformed source point, Mahalanobis
+// matrix.  One warp per source point.
+__global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv, const float4* __restrict__ src,
+                                                                      const double* __restrict__ src_nrm, int n,
+                                                                      const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
+                                                                      float max_corr_sq, int* __restrict__ corr,
+                                                                      double* __restrict__ maha) {
+  __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  WarpList wl = make_warp_list(s_list, warp);
+  for (int i = blockIdx.x * kRegWarps + warp; i < n; i += gridDim.x * kRegWarps) {
+    const float3 q = xform(Tf, __ldg(src + i));
+    Neighbor nb;
+    const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, max_corr_sq, wl, nb);
+    const float d2 = __shfl_sync(kFull, nb.d2, 0);
+    const int id = __shfl_sync(kFull, nb.id, 0);
+    if (lane != 0) continue;
+    const int c = (nf > 0 && d2 < max_corr_sq) ? id : -1;
+    corr[i] = c;
+    if (c >= 0) gicp_store_maha(src_nrm, tgt_nrm, i, c, T, maha);
+  }
+}
+
+// update_correspondences, batched shape: one thread per source point (nn1_exact_thread)
+__global__ void __launch_bounds__(256) gicp_corr_thread_kernel(MapView mv, const float4* __restrict__ src, const double* __restrict__ src_nrm,
+                                                               int n, const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
+                                                               float max_corr_sq, int* __restrict__ corr, double* __restrict__ maha) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float3 q = xform(Tf, __ldg(src + i));
+  float d2; int id;
+  const bool f = nn1_exact_thread(mv, q.x, q.y, q.z, max_corr_sq, &d2, &id);
+  const int c = (f && d2 < max_corr_sq) ? id : -1;
+  corr[i] = c;
+  if (c >= 0) gicp_store_maha(src_nrm, tgt_nrm, i, c, T, maha);
+}
+
+// One distribution-to-distribution residual e at the transformed point t with Mahalanobis matrix M, weighted by w:
+// e^T M e into vals[27] and, with deriv, J^T M J (upper triangle) into vals[0..21) and J^T M e into vals[21..27), with
+// J = d(t)/d(rotation, translation).  GICP passes w = 1.0 (an exact product), VGICP sqrt(voxel points).
+__device__ __forceinline__ void accum_d2d(double (&vals)[29], const double (&M)[3][3], const double3 e, const double3 t, double w,
+                                          bool deriv) {
+  const double cx = M[0][0] * e.x + M[0][1] * e.y + M[0][2] * e.z, cy = M[1][0] * e.x + M[1][1] * e.y + M[1][2] * e.z,
+               cz = M[2][0] * e.x + M[2][1] * e.y + M[2][2] * e.z;
+  vals[27] += w * (e.x * cx + e.y * cy + e.z * cz);
+  if (deriv) {
+    const double J[3][6] = {{0., -t.z, t.y, -1., 0., 0.}, {t.z, 0., -t.x, 0., -1., 0.}, {-t.y, t.x, 0., 0., 0., -1.}};
+    double MJ[3][6];
+#pragma unroll
+    for (int cc = 0; cc < 6; cc++) {
+      MJ[0][cc] = M[0][0] * J[0][cc] + M[0][1] * J[1][cc] + M[0][2] * J[2][cc];
+      MJ[1][cc] = M[1][0] * J[0][cc] + M[1][1] * J[1][cc] + M[1][2] * J[2][cc];
+      MJ[2][cc] = M[2][0] * J[0][cc] + M[2][1] * J[1][cc] + M[2][2] * J[2][cc];
+    }
+    int q = 0;
+#pragma unroll
+    for (int p = 0; p < 6; p++) {
+#pragma unroll
+      for (int r = p; r < 6; r++) vals[q++] += w * (J[0][p] * MJ[0][r] + J[1][p] * MJ[1][r] + J[2][p] * MJ[2][r]);
+      vals[21 + p] += w * (J[0][p] * cx + J[1][p] * cy + J[2][p] * cz);
+    }
+  }
+}
+
 // linearize / compute_error (fast_gicp_impl.hpp:159-242), one thread per source point, double.
 template <bool DERIV>
 __global__ void __launch_bounds__(256) gicp_cost_kernel(const float4* __restrict__ src, int n, const float4* __restrict__ tgt,
@@ -446,34 +465,12 @@ __global__ void __launch_bounds__(256) gicp_cost_kernel(const float4* __restrict
     const int c = corr[i];
     if (c < 0) continue;
     vals[28] += 1.0;
-    const float4 a = __ldg(src + i), b = __ldg(tgt + c);
-    const double ax = a.x, ay = a.y, az = a.z;
-    const double tx = T.R[0] * ax + T.R[1] * ay + T.R[2] * az + T.t[0];
-    const double ty = T.R[3] * ax + T.R[4] * ay + T.R[5] * az + T.t[1];
-    const double tz = T.R[6] * ax + T.R[7] * ay + T.R[8] * az + T.t[2];
-    const double ex = (double)b.x - tx, ey = (double)b.y - ty, ez = (double)b.z - tz;
+    const float4 b = __ldg(tgt + c);
+    const double3 t = xform(T, __ldg(src + i));
+    const double3 e = make_double3((double)b.x - t.x, (double)b.y - t.y, (double)b.z - t.z);
     const double* Ms = maha + 6 * (size_t)i;
     const double M[3][3] = {{Ms[0], Ms[1], Ms[2]}, {Ms[1], Ms[3], Ms[4]}, {Ms[2], Ms[4], Ms[5]}};
-    const double cx = M[0][0] * ex + M[0][1] * ey + M[0][2] * ez, cy = M[1][0] * ex + M[1][1] * ey + M[1][2] * ez,
-                 cz = M[2][0] * ex + M[2][1] * ey + M[2][2] * ez;
-    vals[27] += ex * cx + ey * cy + ez * cz;
-    if (DERIV) {
-      const double J[3][6] = {{0., -tz, ty, -1., 0., 0.}, {tz, 0., -tx, 0., -1., 0.}, {-ty, tx, 0., 0., 0., -1.}};
-      double MJ[3][6];
-#pragma unroll
-      for (int cc = 0; cc < 6; cc++) {
-        MJ[0][cc] = M[0][0] * J[0][cc] + M[0][1] * J[1][cc] + M[0][2] * J[2][cc];
-        MJ[1][cc] = M[1][0] * J[0][cc] + M[1][1] * J[1][cc] + M[1][2] * J[2][cc];
-        MJ[2][cc] = M[2][0] * J[0][cc] + M[2][1] * J[1][cc] + M[2][2] * J[2][cc];
-      }
-      int q = 0;
-#pragma unroll
-      for (int p = 0; p < 6; p++) {
-#pragma unroll
-        for (int r = p; r < 6; r++) vals[q++] += J[0][p] * MJ[0][r] + J[1][p] * MJ[1][r] + J[2][p] * MJ[2][r];
-        vals[21 + p] += J[0][p] * cx + J[1][p] * cy + J[2][p] * cz;
-      }
-    }
+    accum_d2d(vals, M, e, t, 1.0, DERIV);
   }
   block_partials<29>(vals, partials);
   grid_finalize<29>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
@@ -501,23 +498,13 @@ __global__ void __launch_bounds__(256) vgicp_accum_kernel(NdtBuildLine* __restri
   const double x = p.x, y = p.y, z = p.z;
   const int3 c = vg_coord(x, y, z, res);
   if (!coord_ok(c.x, c.y, c.z)) { atomicAdd(fail, 1u); return; }
-  const unsigned long long key = pack_key(c.x, c.y, c.z, 0);
+  const long long s = claim_slot(tab, mask, pack_key(c.x, c.y, c.z, 0));
+  if (s < 0) { atomicAdd(fail, 1u); return; }
   const double nx = nrm[4 * (size_t)i], ny = nrm[4 * (size_t)i + 1], nz = nrm[4 * (size_t)i + 2];
-  unsigned long long s = hash_key(key) & mask;
-  for (unsigned probe = 0; probe < kMaxProbe; probe++) {
-    unsigned long long* kp = &tab[s].key;
-    unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(kp);
-    if (cur == 0ull) cur = atomicCAS(kp, 0ull, key), cur = cur == 0ull ? key : cur;
-    if (cur == key) {
-      atomicAdd(&tab[s].count, 1u);
-      atomicAdd(&tab[s].sum[0], x); atomicAdd(&tab[s].sum[1], y); atomicAdd(&tab[s].sum[2], z);
-      atomicAdd(&tab[s].sxx[0], 1.0 - 0.999 * nx * nx); atomicAdd(&tab[s].sxx[1], -0.999 * nx * ny); atomicAdd(&tab[s].sxx[2], -0.999 * nx * nz);
-      atomicAdd(&tab[s].sxx[3], 1.0 - 0.999 * ny * ny); atomicAdd(&tab[s].sxx[4], -0.999 * ny * nz); atomicAdd(&tab[s].sxx[5], 1.0 - 0.999 * nz * nz);
-      return;
-    }
-    s = (s + 1) & mask;
-  }
-  atomicAdd(fail, 1u);
+  atomicAdd(&tab[s].count, 1u);
+  atomicAdd(&tab[s].sum[0], x); atomicAdd(&tab[s].sum[1], y); atomicAdd(&tab[s].sum[2], z);
+  atomicAdd(&tab[s].sxx[0], 1.0 - 0.999 * nx * nx); atomicAdd(&tab[s].sxx[1], -0.999 * nx * ny); atomicAdd(&tab[s].sxx[2], -0.999 * nx * nz);
+  atomicAdd(&tab[s].sxx[3], 1.0 - 0.999 * ny * ny); atomicAdd(&tab[s].sxx[4], -0.999 * ny * nz); atomicAdd(&tab[s].sxx[5], 1.0 - 0.999 * nz * nz);
 }
 
 // AdditiveGaussianVoxel::finalize
@@ -540,19 +527,6 @@ __global__ void __launch_bounds__(256) vgicp_finalize_kernel(const NdtBuildLine*
   out[s] = o;
 }
 
-__device__ __forceinline__ int vg_lookup(const VgView& v, int x, int y, int z) {
-  if (!coord_ok(x, y, z)) return -1;
-  const unsigned long long key = pack_key(x, y, z, 0);
-  unsigned long long s = hash_key(key) & v.mask;
-  for (unsigned probe = 0; probe < kMaxProbe; probe++) {
-    const unsigned long long k = __ldg(&v.lines[s].key);
-    if (k == key) return (int)s;
-    if (k == 0ull) return -1;
-    s = (s + 1) & v.mask;
-  }
-  return -1;
-}
-
 // linearize (UPDATE: update_correspondences at T, Mahalanobis matrices stored) / compute_error (reuse).
 // One thread per source point, double.
 template <bool UPDATE, bool DERIV>
@@ -566,15 +540,11 @@ __global__ void __launch_bounds__(256) vgicp_cost_kernel(VgView v, const float4*
   for (int j = 0; j < 29; j++) vals[j] = 0.0;
 #pragma unroll 1
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 a = __ldg(src + i);
-    const double ax = a.x, ay = a.y, az = a.z;
-    const double tx = T.R[0] * ax + T.R[1] * ay + T.R[2] * az + T.t[0];
-    const double ty = T.R[3] * ax + T.R[4] * ay + T.R[5] * az + T.t[1];
-    const double tz = T.R[6] * ax + T.R[7] * ay + T.R[8] * az + T.t[2];
+    const double3 t = xform(T, __ldg(src + i));
     int3 c = make_int3(0, 0, 0);
     double rn[3] = {0.0, 0.0, 0.0};
     if (UPDATE) {
-      c = vg_coord(tx, ty, tz, v.res);
+      c = vg_coord(t.x, t.y, t.z, v.res);
       const double* na = src_nrm + 4 * (size_t)i;
       rn[0] = T.R[0] * na[0] + T.R[1] * na[1] + T.R[2] * na[2];
       rn[1] = T.R[3] * na[0] + T.R[4] * na[1] + T.R[5] * na[2];
@@ -585,10 +555,8 @@ __global__ void __launch_bounds__(256) vgicp_cost_kernel(VgView v, const float4*
       const size_t q = (size_t)o * n + i;
       int slot;
       if (UPDATE) {
-        int ox, oy, oz;
-        if (n_off == 27) { ox = o / 9 - 1; oy = (o / 3) % 3 - 1; oz = o % 3 - 1; }
-        else { ox = c_ndt_off7[o][0]; oy = c_ndt_off7[o][1]; oz = c_ndt_off7[o][2]; }
-        slot = vg_lookup(v, c.x + ox, c.y + oy, c.z + oz);
+        const int3 d = stencil_offset(o, n_off);
+        slot = voxel_lookup(v, c.x + d.x, c.y + d.y, c.z + d.z);
         corr[q] = slot;
       } else {
         slot = corr[q];
@@ -613,56 +581,62 @@ __global__ void __launch_bounds__(256) vgicp_cost_kernel(VgView v, const float4*
         M[0][0] = Ms[0]; M[0][1] = M[1][0] = Ms[1]; M[0][2] = M[2][0] = Ms[2]; M[1][1] = Ms[3]; M[1][2] = M[2][1] = Ms[4]; M[2][2] = Ms[5];
       }
       const double w = sqrt((double)ln->n);
-      const double ex = ln->mean[0] - tx, ey = ln->mean[1] - ty, ez = ln->mean[2] - tz;
-      const double cx = M[0][0] * ex + M[0][1] * ey + M[0][2] * ez, cy = M[1][0] * ex + M[1][1] * ey + M[1][2] * ez,
-                   cz = M[2][0] * ex + M[2][1] * ey + M[2][2] * ez;
-      vals[27] += w * (ex * cx + ey * cy + ez * cz);
-      if (DERIV) {
-        const double J[3][6] = {{0., -tz, ty, -1., 0., 0.}, {tz, 0., -tx, 0., -1., 0.}, {-ty, tx, 0., 0., 0., -1.}};
-        double MJ[3][6];
-#pragma unroll
-        for (int cc = 0; cc < 6; cc++) {
-          MJ[0][cc] = M[0][0] * J[0][cc] + M[0][1] * J[1][cc] + M[0][2] * J[2][cc];
-          MJ[1][cc] = M[1][0] * J[0][cc] + M[1][1] * J[1][cc] + M[1][2] * J[2][cc];
-          MJ[2][cc] = M[2][0] * J[0][cc] + M[2][1] * J[1][cc] + M[2][2] * J[2][cc];
-        }
-        int qq = 0;
-#pragma unroll
-        for (int p = 0; p < 6; p++) {
-#pragma unroll
-          for (int r = p; r < 6; r++) vals[qq++] += w * (J[0][p] * MJ[0][r] + J[1][p] * MJ[1][r] + J[2][p] * MJ[2][r]);
-          vals[21 + p] += w * (J[0][p] * cx + J[1][p] * cy + J[2][p] * cz);
-        }
-      }
+      accum_d2d(vals, M, make_double3(ln->mean[0] - t.x, ln->mean[1] - t.y, ln->mean[2] - t.z), t, w, DERIV);
     }
   }
   block_partials<29>(vals, partials);
   grid_finalize<29>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
 
-// getFitnessScore: sum of squared 1-NN distances <= max_range, and their count.  One warp per point.
-__global__ void __launch_bounds__(kRegWarps * 32, 3) fitness_kernel(MapView mv, const float4* __restrict__ src, int n, Pose34f Tf,
-                                                                    float search_sq, float max_range, double* __restrict__ partials,
-                                                                    unsigned* __restrict__ done, double* __restrict__ result,
-                                                                    double seq, ShardComm sc) {
-  __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
+// Exact nearest-neighbour distance by a scan of the whole target, for points with nothing inside the grid search radius:
+// calc_fitness_score counts every point however far (max_range = DBL_MAX).  Thread version.
+__device__ __forceinline__ float nn_scan_thread(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz) {
+  float bd = 3.0e38f;
+  for (int j = 0; j < n_tgt; j++) { const float4 b = __ldg(tgt + j); bd = fminf(bd, dist2(qx, qy, qz, b.x, b.y, b.z)); }
+  return bd;
+}
+// Warp version: lanes stride over the target, then a min across lanes (every lane returns it).
+__device__ __forceinline__ float nn_scan_warp(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz) {
+  float bd = 3.0e38f;
+  for (int j = threadIdx.x & 31; j < n_tgt; j += 32) { const float4 b = __ldg(tgt + j); bd = fminf(bd, dist2(qx, qy, qz, b.x, b.y, b.z)); }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) bd = fminf(bd, __shfl_xor_sync(0xffffffffu, bd, o));
+  return bd;
+}
+
+// getFitnessScore (sum of squared 1-NN distances <= max_range, and their count) over block lb of the G blocks a cloud of n
+// points gets, stored as the block's row (sum, count) of partials.  WARP: one warp per point (knn_exact_warp), else one
+// thread per point (nn1_exact_thread).  tgt != nullptr: points with no neighbour within search_sq get the exact one by a
+// scan of the whole target (nn_scan_*), for calc_fitness_score.  The single-pair kernel and the loop detector's batched
+// kernel (loop.cu) both run this body, so a candidate's row has the single-pair bits.
+template <bool WARP>
+__device__ __forceinline__ void fitness_range(const MapView& mv, const float4* __restrict__ src, int n, int lb, int G, const Pose34f& Tf,
+                                              float search_sq, float max_range, const float4* __restrict__ tgt, int n_tgt,
+                                              double* __restrict__ partials) {
   __shared__ double s_acc[kRegWarps][2];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  WarpList wl;
-  wl.d = reinterpret_cast<unsigned*>(s_list + warp * kWarpListBytes);
-  wl.id = reinterpret_cast<int*>(wl.d + kCandCap);
-  wl.loc = reinterpret_cast<unsigned*>(wl.id + kCandCap);
-  wl.n = 0;
   double sum = 0.0, cnt = 0.0;
-  for (int i = blockIdx.x * kRegWarps + warp; i < n; i += gridDim.x * kRegWarps) {
-    const float4 a = __ldg(src + i);
-    const float qx = Tf.R[0] * a.x + Tf.R[1] * a.y + Tf.R[2] * a.z + Tf.t[0];
-    const float qy = Tf.R[3] * a.x + Tf.R[4] * a.y + Tf.R[5] * a.z + Tf.t[1];
-    const float qz = Tf.R[6] * a.x + Tf.R[7] * a.y + Tf.R[8] * a.z + Tf.t[2];
-    Neighbor nb;
-    const int nf = knn_exact_warp<1>(mv, qx, qy, qz, search_sq, wl, nb);
-    const float d2 = __shfl_sync(kFull, nb.d2, 0);
-    if (nf > 0 && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
+  if constexpr (WARP) {
+    __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
+    WarpList wl = make_warp_list(s_list, warp);
+    for (int i = lb * kRegWarps + warp; i < n; i += G * kRegWarps) {
+      const float3 q = xform(Tf, __ldg(src + i));
+      Neighbor nb;
+      const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, search_sq, wl, nb);
+      float d2 = __shfl_sync(kFull, nb.d2, 0);
+      bool found = nf > 0;
+      if (!found && tgt) { d2 = nn_scan_warp(tgt, n_tgt, q.x, q.y, q.z); found = n_tgt > 0; }   // warp-uniform
+      if (found && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
+    }
+  } else {
+    for (int i = lb * blockDim.x + threadIdx.x; i < n; i += G * blockDim.x) {
+      const float3 q = xform(Tf, __ldg(src + i));
+      float d2; int id;
+      bool found = nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
+      if (!found && tgt) { d2 = nn_scan_thread(tgt, n_tgt, q.x, q.y, q.z); found = n_tgt > 0; }
+      if (found && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
+    }
+    sum = warp_sum(sum); cnt = warp_sum(cnt);
   }
   if (lane == 0) { s_acc[warp][0] = sum; s_acc[warp][1] = cnt; }
   __syncthreads();
@@ -671,32 +645,16 @@ __global__ void __launch_bounds__(kRegWarps * 32, 3) fitness_kernel(MapView mv, 
     for (int w = 0; w < kRegWarps; w++) s += s_acc[w][threadIdx.x];
     partials[(size_t)blockIdx.x * kNV + threadIdx.x] = s;
   }
-  grid_finalize<2>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
 
-// getFitnessScore, batched shape: one thread per source point, block reduction, same last-block fold
-__global__ void __launch_bounds__(256) fitness_thread_kernel(MapView mv, const float4* __restrict__ src, int n, Pose34f Tf, float search_sq,
-                                                             float max_range, double* __restrict__ partials, unsigned* __restrict__ done,
-                                                             double* __restrict__ result, double seq, ShardComm sc) {
-  __shared__ double s_acc[8][2];
-  double sum = 0.0, cnt = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float4 a = __ldg(src + i);
-    const float qx = Tf.R[0] * a.x + Tf.R[1] * a.y + Tf.R[2] * a.z + Tf.t[0];
-    const float qy = Tf.R[3] * a.x + Tf.R[4] * a.y + Tf.R[5] * a.z + Tf.t[1];
-    const float qz = Tf.R[6] * a.x + Tf.R[7] * a.y + Tf.R[8] * a.z + Tf.t[2];
-    float d2; int id;
-    if (nn1_exact_thread(mv, qx, qy, qz, search_sq, &d2, &id) && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
-  }
-  sum = warp_sum(sum); cnt = warp_sum(cnt);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { s_acc[warp][0] = sum; s_acc[warp][1] = cnt; }
-  __syncthreads();
-  if (threadIdx.x < 2) {
-    double s = 0.0;
-    for (int w = 0; w < 8; w++) s += s_acc[w][threadIdx.x];
-    partials[(size_t)blockIdx.x * kNV + threadIdx.x] = s;
-  }
+// getFitnessScore of one cloud: fitness_range over the whole grid, then grid_finalize.  Blocks of kRegWarps warps; the warp
+// shape asks for 3 blocks per SM, the thread shape for no minimum (0).
+template <bool WARP>
+__global__ void __launch_bounds__(kRegWarps * 32, WARP ? 3 : 0) fitness_kernel(MapView mv, const float4* __restrict__ src, int n,
+                                                                               Pose34f Tf, float search_sq, float max_range,
+                                                                               double* __restrict__ partials, unsigned* __restrict__ done,
+                                                                               double* __restrict__ result, double seq, ShardComm sc) {
+  fitness_range<WARP>(mv, src, n, (int)blockIdx.x, (int)gridDim.x, Tf, search_sq, max_range, nullptr, 0, partials);
   grid_finalize<2>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
 
@@ -748,32 +706,34 @@ static void T_to_pose(const double* T, Pose34d* d, Pose34f* f) {
   }
 }
 
-// Spin on the sequence number a reduction kernel publishes into mapped host memory (acquire: the sums stored before it
-// must not be read ahead of it on hosts that reorder loads; bounded, so a hung kernel becomes an error).
-static lsd_status_t wait_seq(const double* h_seq_slot, cudaStream_t stream, double seq) {
-  const unsigned long long* h = reinterpret_cast<const unsigned long long*>(h_seq_slot);
-  unsigned long long want;
-  memcpy(&want, &seq, 8);
-  const auto t0 = std::chrono::steady_clock::now();
-  for (unsigned long long spins = 0;; spins++) {
-    if (__atomic_load_n(h, __ATOMIC_ACQUIRE) == want) return LSD_OK;
-    if ((spins & 0xfff) == 0xfff) {
-      cudaError_t e = cudaStreamQuery(stream);
-      if (e != cudaSuccess && e != cudaErrorNotReady) return cuda_fail(e, "kernel while waiting for the reduction", __FILE__, __LINE__);
-      if (e == cudaSuccess) {
-        if (__atomic_load_n(h, __ATOMIC_ACQUIRE) == want) return LSD_OK;
-        set_error("reduction result never published");
-        return LSD_ERR_CUDA;
-      }
-      if (std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count() > 20.0) { set_error("timed out waiting for a cost evaluation (kernel hung?)"); return LSD_ERR_CUDA; }
-    }
-  }
-}
-static lsd_status_t reg_wait(lsd_reg* r, double seq) { return wait_seq(r->h_result + kResSeq, r->stream, seq); }
+static lsd_status_t reg_wait(lsd_reg* r, double seq) { return wait_seq(r->h_result + kResSeq, r->stream, seq, 20.0); }
 
 constexpr int kThreadShapeMin = 16384;  // clouds from this size on use the thread-per-point search kernels
 static int reg_grid(int n) { return std::max(1, std::min((n + 255) / 256, kLioMaxGrid)); }
 static int warp_grid(int n) { return std::max(1, std::min((n + kRegWarps - 1) / kRegWarps, lsd::kNumSms * 6)); }
+
+// getFitnessScore's grid search radius: max_range, at most 64 map voxels
+static float fitness_search_sq(double max_range, double map_resolution) {
+  return (float)std::min(max_range, 64.0 * map_resolution * map_resolution * 64.0);
+}
+
+// f(std::bool_constant<update>, std::bool_constant<deriv>): launches the <UPDATE, DERIV> instance of a cost kernel
+template <class F>
+static void dispatch_update_deriv(bool update, bool deriv, F&& f) {
+  using Y = std::true_type;
+  using N = std::false_type;
+  if (update && deriv) f(Y{}, Y{});
+  else if (update) f(Y{}, N{});
+  else if (deriv) f(N{}, Y{});
+  else f(N{}, N{});
+}
+
+// H (36, symmetric) and b (6) from a cost row (upper triangle of H in 0..21, b in 21..27)
+static void unpack_hb(const double* res, double* H36, double* b6) {
+  int q = 0;
+  for (int a = 0; a < 6; a++) for (int c = a; c < 6; c++) { H36[6 * a + c] = H36[6 * c + a] = res[q]; q++; }
+  for (int a = 0; a < 6; a++) b6[a] = res[21 + a];
+}
 
 // linearize (update = true) / compute_error at T.  H36/b6 may be null.
 static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H36, double* b6, double* err, int* n_corr) {
@@ -790,10 +750,10 @@ static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H
     T_to_pose(T, nullptr, &ev);
     const int no = r->p.ndt_neighbors;
     const int g = reg_grid(r->n_src);
-    if (update && deriv) ndt_cost_kernel<true, true><<<g, 256, 0, st>>>(r->ndt, r->d_src, r->n_src, no, lin, ev, r->d_corr, r->d_partials, r->d_done, r->d_result, seq, r->sc);
-    else if (update) ndt_cost_kernel<true, false><<<g, 256, 0, st>>>(r->ndt, r->d_src, r->n_src, no, lin, ev, r->d_corr, r->d_partials, r->d_done, r->d_result, seq, r->sc);
-    else if (deriv) ndt_cost_kernel<false, true><<<g, 256, 0, st>>>(r->ndt, r->d_src, r->n_src, no, lin, ev, r->d_corr, r->d_partials, r->d_done, r->d_result, seq, r->sc);
-    else ndt_cost_kernel<false, false><<<g, 256, 0, st>>>(r->ndt, r->d_src, r->n_src, no, lin, ev, r->d_corr, r->d_partials, r->d_done, r->d_result, seq, r->sc);
+    dispatch_update_deriv(update, deriv, [&](auto U, auto D) {
+      ndt_cost_kernel<decltype(U)::value, decltype(D)::value><<<g, 256, 0, st>>>(r->ndt, r->d_src, r->n_src, no, lin, ev, r->d_corr,
+                                                                                 r->d_partials, r->d_done, r->d_result, seq, r->sc);
+    });
     r->launches++;
   } else if (r->p.kind == LSD_REG_VGICP) {
     if (!r->vg.lines || !r->tgt_map_built) { set_error("registration: no target cloud"); return LSD_ERR_INVALID; }
@@ -801,10 +761,10 @@ static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H
     T_to_pose(T, &Td, nullptr);
     const int no = r->p.ndt_neighbors;
     const int g = reg_grid(r->n_src);
-    if (update && deriv) vgicp_cost_kernel<true, true><<<g, 256, 0, st>>>(r->vg, r->d_src, r->d_src_nrm, r->n_src, no, Td, r->d_corr, r->d_maha, r->d_partials, r->d_done, r->d_result, seq, r->sc);
-    else if (update) vgicp_cost_kernel<true, false><<<g, 256, 0, st>>>(r->vg, r->d_src, r->d_src_nrm, r->n_src, no, Td, r->d_corr, r->d_maha, r->d_partials, r->d_done, r->d_result, seq, r->sc);
-    else if (deriv) vgicp_cost_kernel<false, true><<<g, 256, 0, st>>>(r->vg, r->d_src, r->d_src_nrm, r->n_src, no, Td, r->d_corr, r->d_maha, r->d_partials, r->d_done, r->d_result, seq, r->sc);
-    else vgicp_cost_kernel<false, false><<<g, 256, 0, st>>>(r->vg, r->d_src, r->d_src_nrm, r->n_src, no, Td, r->d_corr, r->d_maha, r->d_partials, r->d_done, r->d_result, seq, r->sc);
+    dispatch_update_deriv(update, deriv, [&](auto U, auto D) {
+      vgicp_cost_kernel<decltype(U)::value, decltype(D)::value><<<g, 256, 0, st>>>(r->vg, r->d_src, r->d_src_nrm, r->n_src, no, Td, r->d_corr,
+                                                                                   r->d_maha, r->d_partials, r->d_done, r->d_result, seq, r->sc);
+    });
     r->launches++;
   } else {
     if (!r->tgt_map_built) { set_error("registration: no target cloud"); return LSD_ERR_INVALID; }
@@ -829,11 +789,7 @@ static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H
   lsd_status_t w = reg_wait(r, seq);
   if (w) return w;
   const double* res = r->h_result;
-  if (H36) {
-    int q = 0;
-    for (int a = 0; a < 6; a++) for (int c = a; c < 6; c++) { H36[6 * a + c] = H36[6 * c + a] = res[q]; q++; }
-    for (int a = 0; a < 6; a++) b6[a] = res[21 + a];
-  }
+  if (H36) unpack_hb(res, H36, b6);
   if (err) *err = res[27];
   if (n_corr) *n_corr = (int)(res[28] + 0.5);
   return LSD_OK;
@@ -1067,6 +1023,44 @@ static lsd_status_t reg_alloc_src(lsd_reg* r, int n) {
   return LSD_OK;
 }
 
+static int auto_log2(size_t n_items, int lo, int hi) {
+  int l = lo;
+  while (l < hi && (1ull << l) < n_items * 2) l++;
+  return l;
+}
+
+// The target's voxel map v (NdtView or VgView, v.res already set) for n points: sized from n (or map_log2_lines), its
+// build table allocated and cleared, accum(build, mask, d_fail) and finalize(build, lines, d_vox) launched on the
+// handle's stream.  Fails with LSD_ERR_CAPACITY when a point found no slot or lies outside the key range.
+template <class View, class Accum, class Finalize>
+static lsd_status_t build_voxel_table(lsd_reg* r, int n, const char* method, View& v, unsigned long long& n_lines, Accum accum,
+                                      Finalize finalize) {
+  cudaStream_t st = r->stream;
+  const int l2 = r->p.map_log2_lines > 0 ? r->p.map_log2_lines : auto_log2((size_t)n / 2 + 1024, 12, 27);
+  const unsigned long long lines = 1ull << l2;
+  NdtBuildLine* build = nullptr;
+  LSD_CUDA(cudaMalloc((void**)&build, lines * sizeof(NdtBuildLine)));
+  LSD_CUDA(cudaMemsetAsync(build, 0, lines * sizeof(NdtBuildLine), st));
+  if (n_lines != lines) {
+    cudaFree(v.lines); v.lines = nullptr;
+    LSD_CUDA(cudaMalloc((void**)&v.lines, lines * sizeof(*v.lines)));
+    n_lines = lines;
+  }
+  v.mask = lines - 1;
+  unsigned* d_cnt = reinterpret_cast<unsigned*>(r->d_done) + 4;
+  LSD_CUDA(cudaMemsetAsync(d_cnt, 0, 8, st));
+  accum(build, lines - 1, d_cnt);
+  finalize(build, lines, d_cnt + 1);
+  r->launches += 2;
+  unsigned h[2] = {0, 0};
+  LSD_CUDA(cudaMemcpyAsync(h, d_cnt, 8, cudaMemcpyDeviceToHost, st));
+  LSD_CUDA(cudaStreamSynchronize(st));
+  LSD_CUDA(cudaFree(build));
+  r->n_voxels = h[1];
+  if (h[0]) { set_error("%s voxel table too small / coordinates out of range: %u points dropped (raise map_log2_lines)", method, h[0]); return LSD_ERR_CAPACITY; }
+  return LSD_OK;
+}
+
 }  // namespace lsd
 
 using namespace lsd;
@@ -1205,12 +1199,6 @@ lsd_status_t lsd_reg_shard_connect(lsd_reg_t* r, const unsigned char* blobs) {
   return LSD_OK;
 }
 
-static int auto_log2(size_t n_items, int lo, int hi) {
-  int l = lo;
-  while (l < hi && (1ull << l) < n_items * 2) l++;
-  return l;
-}
-
 static lsd_status_t build_point_map(lsd_reg* r, lsd_map** mp, const float4* d_pts, int n) {
   const int l2 = r->p.map_log2_lines > 0 ? r->p.map_log2_lines : auto_log2((size_t)n, 12, 26);
   if (*mp && (*mp)->n_lines == (1ull << l2)) {
@@ -1250,29 +1238,15 @@ lsd_status_t lsd_reg_set_target_dev(lsd_reg_t* r, const float* pts_dev, int n) {
   r->n_tgt = n;
   r->tgt_map_built = false;
   if (r->p.kind == LSD_REG_NDT_P2D) {
-    const int l2 = r->p.map_log2_lines > 0 ? r->p.map_log2_lines : auto_log2((size_t)n / 2 + 1024, 12, 27);
-    const unsigned long long lines = 1ull << l2;
-    NdtBuildLine* build = nullptr;
-    LSD_CUDA(cudaMalloc((void**)&build, lines * sizeof(NdtBuildLine)));
-    LSD_CUDA(cudaMemsetAsync(build, 0, lines * sizeof(NdtBuildLine), st));
-    if (r->ndt_lines != lines) {
-      cudaFree(r->ndt.lines); r->ndt.lines = nullptr;
-      LSD_CUDA(cudaMalloc((void**)&r->ndt.lines, lines * sizeof(NdtLine)));
-      r->ndt_lines = lines;
-    }
-    r->ndt.mask = lines - 1;
     r->ndt.res = (float)r->p.resolution;
-    unsigned* d_cnt = reinterpret_cast<unsigned*>(r->d_done) + 4;
-    LSD_CUDA(cudaMemsetAsync(d_cnt, 0, 8, st));
-    ndt_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, lines - 1, r->ndt.res, r->d_tgt, n, d_cnt, r->sc.rank, r->sc.world, r->shard_tile);
-    ndt_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, r->ndt.lines, lines, d_cnt + 1);
-    r->launches += 2;
-    unsigned h[2] = {0, 0};
-    LSD_CUDA(cudaMemcpyAsync(h, d_cnt, 8, cudaMemcpyDeviceToHost, st));
-    LSD_CUDA(cudaStreamSynchronize(st));
-    LSD_CUDA(cudaFree(build));
-    r->n_voxels = h[1];
-    if (h[0]) { set_error("NDT voxel table too small / coordinates out of range: %u points dropped (raise map_log2_lines)", h[0]); return LSD_ERR_CAPACITY; }
+    lsd_status_t s = build_voxel_table(r, n, "NDT", r->ndt, r->ndt_lines,
+        [&](NdtBuildLine* build, unsigned long long mask, unsigned* d_fail) {
+          ndt_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, mask, r->ndt.res, r->d_tgt, n, d_fail, r->sc.rank, r->sc.world, r->shard_tile);
+        },
+        [&](const NdtBuildLine* build, unsigned long long lines, unsigned* d_vox) {
+          ndt_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, r->ndt.lines, lines, d_vox);
+        });
+    if (s) return s;
   } else {
     lsd_status_t s = build_point_map(r, &r->tgt_map, r->d_tgt, n);
     if (s) return s;
@@ -1283,29 +1257,15 @@ lsd_status_t lsd_reg_set_target_dev(lsd_reg_t* r, const float* pts_dev, int n) {
     r->launches += 3;
     r->tgt_map_built = true;
     if (r->p.kind == LSD_REG_VGICP) {  // GaussianVoxelMap::create_voxelmap (built lazily by the reference, fast_vgicp_impl.hpp:121-124)
-      const int l2 = r->p.map_log2_lines > 0 ? r->p.map_log2_lines : auto_log2((size_t)n / 2 + 1024, 12, 27);
-      const unsigned long long lines = 1ull << l2;
-      NdtBuildLine* build = nullptr;
-      LSD_CUDA(cudaMalloc((void**)&build, lines * sizeof(NdtBuildLine)));
-      LSD_CUDA(cudaMemsetAsync(build, 0, lines * sizeof(NdtBuildLine), st));
-      if (r->vg_lines != lines) {
-        cudaFree(r->vg.lines); r->vg.lines = nullptr;
-        LSD_CUDA(cudaMalloc((void**)&r->vg.lines, lines * sizeof(VgLine)));
-        r->vg_lines = lines;
-      }
-      r->vg.mask = lines - 1;
       r->vg.res = r->p.resolution;
-      unsigned* d_cnt = reinterpret_cast<unsigned*>(r->d_done) + 4;
-      LSD_CUDA(cudaMemsetAsync(d_cnt, 0, 8, st));
-      vgicp_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, lines - 1, r->vg.res, r->d_tgt, r->d_tgt_nrm, n, d_cnt);
-      vgicp_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, r->vg.lines, lines, d_cnt + 1);
-      r->launches += 2;
-      unsigned h[2] = {0, 0};
-      LSD_CUDA(cudaMemcpyAsync(h, d_cnt, 8, cudaMemcpyDeviceToHost, st));
-      LSD_CUDA(cudaStreamSynchronize(st));
-      LSD_CUDA(cudaFree(build));
-      r->n_voxels = h[1];
-      if (h[0]) { set_error("VGICP voxel table too small / coordinates out of range: %u points dropped (raise map_log2_lines)", h[0]); return LSD_ERR_CAPACITY; }
+      s = build_voxel_table(r, n, "VGICP", r->vg, r->vg_lines,
+          [&](NdtBuildLine* build, unsigned long long mask, unsigned* d_fail) {
+            vgicp_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, mask, r->vg.res, r->d_tgt, r->d_tgt_nrm, n, d_fail);
+          },
+          [&](const NdtBuildLine* build, unsigned long long lines, unsigned* d_vox) {
+            vgicp_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, r->vg.lines, lines, d_vox);
+          });
+      if (s) return s;
     }
     LSD_CUDA(cudaStreamSynchronize(st));
   }
@@ -1412,19 +1372,19 @@ lsd_status_t lsd_reg_fitness(lsd_reg_t* r, const double* T16_or_null, double max
   Pose34f Tf;
   T_to_pose(T16_or_null ? T16_or_null : r->final_T, nullptr, &Tf);
   const double seq = (double)(++r->seq);
-  const float search_sq = (float)std::min(max_range, 64.0 * r->p.map_resolution * r->p.map_resolution * 64.0);
+  const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
   if (r->n_src >= kThreadShapeMin)
-    fitness_thread_kernel<<<reg_grid(r->n_src), 256, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, (float)max_range,
-                                                              r->d_partials, r->d_done, r->d_result, seq, r->sc);
+    fitness_kernel<false><<<reg_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, (float)max_range,
+                                                                         r->d_partials, r->d_done, r->d_result, seq, r->sc);
   else
-    fitness_kernel<<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, (float)max_range,
-                                                                  r->d_partials, r->d_done, r->d_result, seq, r->sc);
+    fitness_kernel<true><<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, (float)max_range,
+                                                                        r->d_partials, r->d_done, r->d_result, seq, r->sc);
   LSD_CUDA(cudaGetLastError());
   r->launches++;
   lsd_status_t w = reg_wait(r, seq);
   if (w) return w;
   const double sum = r->h_result[0], cnt = r->h_result[1];
-  *score = cnt > 0 ? sum / cnt : 1.7976931348623157e308;
+  *score = cnt > 0 ? sum / cnt : DBL_MAX;
   return LSD_OK;
 }
 

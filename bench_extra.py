@@ -4,6 +4,7 @@
   config[3]  GICP loop-closure batch: submap pairs x 200 k pts (per-GPU share of the 256-pair batch)
   config[4]  detection voxelizer: 200 k pts, 4-frame window
   loop       loop-closure detection: one new key frame vs C candidates (C = 4, 16, 32), ~30 k pts each
+  galign     global-alignment closure search: 72 reference x 100 new key frames, ~13 k pts each, hundreds of pairs
 Prints one JSON object per config with device times (CUDA events via torch on the default stream are
 NOT used: the library runs on its own stream, so wall time around synchronous C-ABI calls is reported)
 and the CPU restatement timed on a bounded sample.
@@ -398,6 +399,79 @@ def loop(args):
         print(json.dumps(out))
 
 
+def galign(args):
+    """Global-alignment closure search: a reference map of R key frames and a new map of M key frames (a second drive around
+    the same loop, plus a stretch in another block).  Batched search against the same (new, reference) pairs run serially
+    through the single-pair kernels on the same tables (serial = 1), and the compiled reference FastVGICP (CPU) on a subset."""
+    import math
+    import lsdreg
+    from lsdreg import synth
+    card = _card()
+    c0, c1 = synth.block_center(0, 0), synth.block_center(1, 0)
+    R_kf, M_kf, M_other, radius = args.galign_refs, args.galign_news, 4, 14.0
+    clouds_ref, clouds_new = [], []
+    for i in range(R_kf):
+        th = 2 * np.pi * i / R_kf
+        clouds_ref.append(synth.scan64(1000 + i, 250, synth.rot_from_rpy(0.0, 0.0, th + np.pi / 2),
+                                       c0 + np.array([radius * np.cos(th), radius * np.sin(th), 0.0])))
+    for j in range(M_kf):
+        th = 2 * np.pi * (j + 0.5) / M_kf
+        clouds_new.append(synth.scan64(2000 + j, 250, synth.rot_from_rpy(0.0, 0.0, th - np.pi / 2),
+                                       c0 + np.array([(radius + 0.8) * np.cos(th), (radius + 0.8) * np.sin(th), 0.0])))
+    for j in range(M_other):
+        clouds_new.append(synth.scan64(3000 + j, 250, np.eye(3), c1 + np.array([4.0 * j - 6.0, -5.0, 0.0]), bi=1))
+    ga = lsdreg.GlobalAligner()
+    refs = [ga.add_keyframe(c, True) for c in clouds_ref]
+    news = [ga.add_keyframe(c, False) for c in clouds_new]
+    cold_ms, closures = t_ms(lambda: ga.search(news))          # first search: builds every table it uses
+    search_ms, closures = t_ms(lambda: ga.search(news), args.galign_reps)
+    st = ga.stats()
+    tried = ga.matches()
+    groups = {}
+    for m in tried:
+        y = np.float32(-m["sc_yaw"])
+        G = np.eye(4)
+        G[0, 0] = G[1, 1] = float(np.float32(math.cos(float(y))))
+        G[1, 0] = float(np.float32(math.sin(float(y)))); G[0, 1] = -G[1, 0]
+        groups.setdefault(m["new_slot"], ([], []))
+        groups[m["new_slot"]][0].append(m["ref_slot"]); groups[m["new_slot"]][1].append(G)
+    def run(serial):
+        return {q: ga.match(q, r, np.array(g), serial=serial) for q, (r, g) in groups.items()}
+    run(False)
+    per_kf_ms, bat = t_ms(lambda: run(False))
+    serial_ms, ser = t_ms(lambda: run(True))
+    same = all(all(np.array_equal(bat[q][k], ser[q][k]) for k in ("final", "converged", "iterations", "fitness")) for q in groups)
+    pairs = len(tried)
+    out = dict(config="global alignment search: %d reference x %d new key frames" % (R_kf, M_kf + M_other), **card,
+               reference_keyframes=R_kf, new_keyframes=M_kf + M_other, pairs=pairs, closures=len(closures),
+               points_per_keyframe=int(np.mean([c.shape[0] for c in clouds_ref + clouds_new])),
+               batched=dict(search_ms=search_ms, first_search_ms=cold_ms, pairs_per_s=pairs / (search_ms * 1e-3), launches=st["launches"],
+                            rounds=st["rounds"], batches=st["batches"], per_keyframe_match_ms=per_kf_ms),
+               serial=dict(ms=serial_ms, pairs_per_s=pairs / (serial_ms * 1e-3), launches=sum(r["launches"] for r in ser.values()),
+                           rounds=sum(r["rounds"] for r in ser.values())),
+               batched_equals_serial=bool(same),
+               # per round and live pair: source point (16 B) + covariance (32 B) + correspondence (4 B) + Mahalanobis (48 B)
+               # + voxel line (128 B) per point, an upper bound reached by the linearising rounds
+               alg_bytes_per_round_max=float(sum(clouds_new[m["new_slot"] - R_kf].shape[0] for m in tried) * (16 + 32 + 4 + 48 + 128)))
+    if not args.no_cpu and os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libref_reg.so")):
+        try:
+            from oracle.reg import RefMatcher
+            sub = tried[:args.galign_ref_pairs]
+            r = RefMatcher("vgicp", resolution=1.0, neighbors=1, max_iterations=64, trans_eps=0.1, rot_eps=0.1, k=20,
+                           nthreads=args.galign_ref_threads)
+            def ref():
+                for m in sub:
+                    G = groups[m["new_slot"]][1][groups[m["new_slot"]][0].index(m["ref_slot"])]
+                    r.set_target(clouds_ref[m["ref_slot"]]); r.set_source(clouds_new[m["new_slot"] - R_kf])
+                    r.align(G); r.fitness(25.0)
+            rm, _ = t_ms(ref)
+            out["reference_fast_vgicp_cpu"] = dict(pairs=len(sub), threads=args.galign_ref_threads, ms=rm, pairs_per_s=len(sub) / (rm * 1e-3))
+        except Exception as e:  # the comparator must never take the measurement down
+            out["reference_fast_vgicp_cpu"] = dict(error=repr(e)[:200])
+    ga.close()
+    print(json.dumps(out))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="ndt,gicp,vfe")
@@ -408,6 +482,11 @@ if __name__ == "__main__":
     ap.add_argument("--gicp-perturb-m", type=float, default=1.0)
     ap.add_argument("--gicp-perturb-deg", type=float, default=5.0)
     ap.add_argument("--loop-reps", type=int, default=5)
+    ap.add_argument("--galign-refs", type=int, default=72)
+    ap.add_argument("--galign-news", type=int, default=96)
+    ap.add_argument("--galign-reps", type=int, default=3)
+    ap.add_argument("--galign-ref-pairs", type=int, default=24)
+    ap.add_argument("--galign-ref-threads", type=int, default=4, help="FastVGICP threads (setNumThreads(4), registrations.cpp:59)")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-ref-cuda", action="store_true", help="skip the legs that time the reference's own CUDA NDT / VGICP (oracle/_ref/libref_cuda*.so)")
     a = ap.parse_args()
@@ -419,6 +498,6 @@ if __name__ == "__main__":
         with contextlib.redirect_stdout(buf):
             lsdreg.init(int(os.environ.get("LOCAL_RANK", 0)))
             for w in a.which.split(","):
-                {"ndt": ndt, "gicp": gicp, "vfe": vfe, "loop": loop}[w](a)
+                {"ndt": ndt, "gicp": gicp, "vfe": vfe, "loop": loop, "galign": galign}[w](a)
     sys.stdout.write(buf.getvalue())
     sys.stdout.flush()

@@ -460,6 +460,90 @@ lsd_status_t lsd_loop_fitness(lsd_loop_t* h, int32_t target_slot, int32_t source
 void lsd_loop_information_matrix(double fitness_score, double* information36);
 
 /* ------------------------------------------------------------------------------------------
+ * Global alignment search — replaces the closure search of global_alignment
+ * (slam/localization/include/global_alignment.hpp:200-258, called from MapLoader::mergeMapSLAM,
+ * slam/localization/src/map_loader.cpp:82-169, when either map has no GNSS origin).  Key-frame clouds (sensor frame) are
+ * uploaded once into a device pool, addressed by slot and marked as reference (the loaded map) or new (the map being
+ * merged); each reference key frame's ScanContext (offset (0, 0), keyframe.cpp:165-167) enters a database in slot order, so
+ * the database index is the reference index.  A reference key frame's point map, k = 20 covariances and VGICP voxel table
+ * are built on its first use as a target and kept; a new key frame's covariances once.  lsd_galign_search does, for all new
+ * key frames given: nine-offset descriptors (:209-214), detectCandidateMatch merged per reference (:215-227), FAST_VGICP of
+ * every (new, reference) pair from yaw2matrix(-sc_yaw) (:231-244) with the Levenberg-Marquardt loops of all pairs
+ * advanced together (one batched cost launch per round), getFitnessScore(25) of all pairs in one launch (:249), and the
+ * gate converged && score < 1.5 (:245-253).  Each pair is bit-identical to the single-pair kernels on the same tables.
+ * The PCM matrix, max-clique and estimate_transform (:261-300) stay with the caller.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct lsd_galign lsd_galign_t;
+typedef struct lsd_galign_params {
+  lsd_reg_params_t reg;             /* lsd_reg_default_params(LSD_REG_VGICP): select_registration_method("FAST_VGICP")
+                                       (registrations.cpp:56-66: res 1.0, eps 0.1 m / 0.1 deg, 64 iterations, k = 20),
+                                       max_process_time_us must be 0                                                     */
+  double sc_dist_thres;             /* 0.30, SC_DIST_THRES (global_alignment.hpp:31)                                    */
+  double icp_score_thres;           /* 1.5, ICP_SCORE_THRES (:32); a closure needs score < this                        */
+  double fitness_score_max_range;   /* 25, FITNESS_SCORE_MAX (:34), SQUARED distance as PCL compares it                */
+  int64_t max_batch_points;         /* pair budget of one batch: sum over its pairs of new-cloud points x ndt_neighbors
+                                       (4 + 48 bytes each for correspondences and Mahalanobis matrices).  A search splits
+                                       into batches of whole new key frames; results do not depend on the split.  2^24 */
+  int sc_db_capacity;               /* reference key frames the ScanContext database holds (4096)                       */
+} lsd_galign_params_t;
+
+typedef struct lsd_galign_closure {
+  int32_t ref_slot, new_slot;  /* Closures(key1 = reference key frame, key2 = new key frame) (:251)                 */
+  float relpose16[16];         /* registration->getFinalTransformation(), row-major: new key frame -> reference   */
+  double score;                /* getFitnessScore(fitness_score_max_range) (:249)                                 */
+  float sc_dist, sc_yaw;       /* the merged SCMatch: distance and yaw (rad) of the ScanContext match             */
+} lsd_galign_closure_t;
+
+typedef struct lsd_galign_match {
+  int32_t new_slot, ref_slot;
+  float sc_dist, sc_yaw;
+  int32_t converged, iterations;
+  double score;                /* getFitnessScore at the final pose (computed for every pair)                      */
+  int32_t accepted;            /* converged && score < icp_score_thres                                            */
+} lsd_galign_match_t;
+
+void lsd_galign_default_params(lsd_galign_params_t* p);
+lsd_status_t lsd_galign_create(lsd_galign_t** out, const lsd_galign_params_t* p);
+lsd_status_t lsd_galign_destroy(lsd_galign_t* h);
+/* KeyFrame::mPoints ([n,4], sensor frame) uploaded once; reference != 0 adds it to the reference map (and its
+ * ScanContext to the database), else to the new map.  *slot = 0, 1, 2, ... in call order. */
+lsd_status_t lsd_galign_add_keyframe(lsd_galign_t* h, const float* xyzi_host, int n, int reference, int32_t* slot);
+/* The search of :206-258 for the new key frames new_slots (in that order).  Writes up to cap closures, ordered by new key
+ * frame, then ascending reference index; *n_closures = closures found (may exceed cap). */
+lsd_status_t lsd_galign_search(lsd_galign_t* h, const int32_t* new_slots, int n_new, lsd_galign_closure_t* out, int cap,
+                               int* n_closures);
+/* Sets max_batch_points (> 0) for the following searches: the memory a search may hold for correspondences and Mahalanobis
+ * matrices at once.  Results do not depend on it. */
+lsd_status_t lsd_galign_set_max_batch_points(lsd_galign_t* h, int64_t max_batch_points);
+/* Every pair the last lsd_galign_search aligned, in its order.  out may be NULL. */
+lsd_status_t lsd_galign_last_matches(lsd_galign_t* h, lsd_galign_match_t* out, int cap, int* n);
+/* Work of the last lsd_galign_search: kernel launches of the matching (tables, cost rounds, fitness), host round trips
+ * (batched cost evaluations), batches.  Any output may be NULL. */
+lsd_status_t lsd_galign_last_stats(lsd_galign_t* h, long long* launches, int* rounds, int* batches);
+/* Lines :215-227 alone, pure host (works without a device): the output of lsd_sc_query for n_off offsets
+ * (cand_idx / cand_dist / cand_shift [n_off][10], n_cand [n_off]) filtered by dist < dist_thres (detectCandidateMatch,
+ * Scancontext.cpp:354) and merged per database index: the smaller float sc_dist wins, the first seen on a tie
+ * (std::map<int, SCMatch>).  Out: ascending index, with float distance and yaw; *n_out = matches (may exceed cap). */
+lsd_status_t lsd_galign_merge_candidates(const int32_t* cand_idx, const double* cand_dist, const int32_t* cand_shift,
+                                         const int32_t* n_cand, int n_off, double dist_thres, int32_t* idx_out,
+                                         float* dist_out, float* yaw_out, int cap, int* n_out);
+/* Parity tap: FAST_VGICP of new_slot against each of ref_slots[n] from guesses16 (double [n,16]), then getFitnessScore.
+ * serial = 0: batched as in lsd_galign_search; serial = 1: the same pairs one after another through the single-pair
+ * kernels of lsd_reg on this handle's tables (the bit-exactness reference).  Per pair: final pose (double [n,16]),
+ * converged, iterations, fitness.  Any output may be NULL.  *launches / *rounds: kernel launches and host round trips
+ * (cost evaluations) of the matching. */
+lsd_status_t lsd_galign_match(lsd_galign_t* h, int32_t new_slot, const int32_t* ref_slots, const double* guesses16, int n,
+                              int serial, double* final16, int32_t* converged, int32_t* iterations, double* fitness,
+                              long long* launches, int* rounds);
+/* The LM iteration log of pair i of the last lsd_galign_match, same layout as lsd_reg_iteration_log. */
+lsd_status_t lsd_galign_iteration_log(lsd_galign_t* h, int i, double* out4_per_iter, int cap_iters, int* n_iters);
+/* One VGICP cost evaluation of new_slot against ref_slot at T16 through the batched kernel (parity tap, as lsd_reg_cost):
+ * update != 0 = linearize (correspondences refreshed), else compute_error with the correspondences of the last update of
+ * this pair.  H36 / b6 may be NULL. */
+lsd_status_t lsd_galign_cost(lsd_galign_t* h, int32_t new_slot, int32_t ref_slot, const double* T16, int update, double* H36,
+                             double* b6, double* err, int* n_corr);
+
+/* ------------------------------------------------------------------------------------------
  * Detection voxelizer (config 5) — replaces sensor_driver/inference/voxelize:
  * Preprocess::forward (preprocess_kernel.cu:56-101: sliding window of max_frame_num frames, older frames
  * re-projected by a 3x4 motion, time channel + 0.1) and Voxelization::forward (voxelization_kernel.cu:

@@ -11,5 +11,5 @@ from .capi import (  # noqa: F401
     STENCIL_NEARBY74, HashVoxelMap, Matcher, Voxelizer, eskf_update_table, LioFrontend, LsdError, VoxelGrid, init, init_cov, lib, make_state,
     state_boxminus, state_boxplus, ImuProcess, eskf_predict, IMU_INITIALIZING, keyframe_filter, LocalMap, LOCALMAP_NONE, keyframe_save, keyframe_load, ERR_IO, ScanContext, FastLio,
     LoopDetector, find_loop_candidates, loop_information_matrix, LOOP_SKIPPED, LOOP_NO_CANDIDATES, LOOP_COARSE_REJECT,
-    LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND)
+    LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND, GlobalAligner, galign_merge_candidates)
 from . import capi  # noqa: F401

@@ -70,6 +70,21 @@ class LoopReport(C.Structure):
                 ("best_score", C.c_double)]
 
 
+class GalignParams(C.Structure):
+    _fields_ = [("reg", RegParams), ("sc_dist_thres", C.c_double), ("icp_score_thres", C.c_double),
+                ("fitness_score_max_range", C.c_double), ("max_batch_points", C.c_int64), ("sc_db_capacity", C.c_int)]
+
+
+class GalignClosure(C.Structure):
+    _fields_ = [("ref_slot", C.c_int32), ("new_slot", C.c_int32), ("relpose16", C.c_float * 16), ("score", C.c_double),
+                ("sc_dist", C.c_float), ("sc_yaw", C.c_float)]
+
+
+class GalignMatch(C.Structure):
+    _fields_ = [("new_slot", C.c_int32), ("ref_slot", C.c_int32), ("sc_dist", C.c_float), ("sc_yaw", C.c_float),
+                ("converged", C.c_int32), ("iterations", C.c_int32), ("score", C.c_double), ("accepted", C.c_int32)]
+
+
 # what LoopDetector.detect decided for each new key frame (LSD_LOOP_*)
 LOOP_SKIPPED, LOOP_NO_CANDIDATES, LOOP_COARSE_REJECT, LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND = range(6)
 
@@ -176,6 +191,18 @@ SIGNATURES = [
     ("lsd_loop_iteration_log", _i, [_vp, _i, _vp, _i, _pi]),
     ("lsd_loop_fitness", _i, [_vp, C.c_int32, C.c_int32, _vp, _d, C.POINTER(_d), _pi]),
     ("lsd_loop_information_matrix", None, [_d, _vp]),
+    ("lsd_galign_default_params", None, [C.POINTER(GalignParams)]),
+    ("lsd_galign_create", _i, [_pp, C.POINTER(GalignParams)]),
+    ("lsd_galign_destroy", _i, [_vp]),
+    ("lsd_galign_add_keyframe", _i, [_vp, _vp, _i, _i, C.POINTER(C.c_int32)]),
+    ("lsd_galign_search", _i, [_vp, _vp, _i, _vp, _i, _pi]),
+    ("lsd_galign_last_matches", _i, [_vp, _vp, _i, _pi]),
+    ("lsd_galign_last_stats", _i, [_vp, C.POINTER(C.c_longlong), _pi, _pi]),
+    ("lsd_galign_set_max_batch_points", _i, [_vp, C.c_int64]),
+    ("lsd_galign_merge_candidates", _i, [_vp, _vp, _vp, _vp, _i, _d, _vp, _vp, _vp, _i, _pi]),
+    ("lsd_galign_match", _i, [_vp, C.c_int32, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, C.POINTER(C.c_longlong), _pi]),
+    ("lsd_galign_iteration_log", _i, [_vp, _i, _vp, _i, _pi]),
+    ("lsd_galign_cost", _i, [_vp, C.c_int32, C.c_int32, _vp, _i, _vp, _vp, C.POINTER(_d), _pi]),
     ("lsd_vfe_default_params", None, [C.POINTER(VfeParams)]),
     ("lsd_vfe_create", _i, [_pp, C.POINTER(VfeParams)]),
     ("lsd_vfe_destroy", _i, [_vp]),
@@ -728,6 +755,118 @@ def loop_information_matrix(fitness_score: float) -> np.ndarray:
     out = np.zeros((6, 6))
     lib.lsd_loop_information_matrix(float(fitness_score), _ptr(out))
     return out
+
+
+def _galign_params(**kw) -> GalignParams:
+    p = GalignParams()
+    lib.lsd_galign_default_params(C.byref(p))
+    for k, v in kw.items():
+        if hasattr(p.reg, k) and not hasattr(p, k):
+            setattr(p.reg, k, v)
+        else:
+            setattr(p, k, v)
+    return p
+
+
+class GlobalAligner:
+    """The closure search of global_alignment (global_alignment.hpp:200-258) on the device: reference and new key frames
+    are added once (clouds stay in device memory, addressed by slot); search() finds the ScanContext matches of each new
+    key frame, aligns all (new, reference) pairs with batched FAST_VGICP and returns the closures that converged with a
+    fitness score below 1.5.  Keyword arguments set lsd_galign_params_t fields or, by name, its matcher parameters."""
+
+    def __init__(self, **kw):
+        self.h = None
+        self.params = _galign_params(**kw)
+        self.h = C.c_void_p()
+        check(lib.lsd_galign_create(C.byref(self.h), C.byref(self.params)))
+
+    def close(self):
+        if self.h:
+            lib.lsd_galign_destroy(self.h)
+        self.h = None
+
+    __del__ = close
+
+    def add_keyframe(self, pts, reference: bool) -> int:
+        pts = _f32(pts)
+        slot = C.c_int32()
+        check(lib.lsd_galign_add_keyframe(self.h, _ptr(pts), pts.shape[0], int(bool(reference)), C.byref(slot)))
+        return slot.value
+
+    def search(self, new_slots) -> list[dict]:
+        """Closures of the new key frames `new_slots`: ordered by new key frame, then ascending reference key frame."""
+        ns = _slots(new_slots)
+        cap = max(90 * ns.size, 1)   # at most 9 offsets x 10 ScanContext candidates per new key frame
+        out = (GalignClosure * cap)()
+        n = C.c_int()
+        check(lib.lsd_galign_search(self.h, _ptr(ns), ns.size, out, cap, C.byref(n)))
+        return [dict(ref_slot=c.ref_slot, new_slot=c.new_slot, relpose=np.array(c.relpose16, np.float32).reshape(4, 4),
+                     score=c.score, sc_dist=c.sc_dist, sc_yaw=c.sc_yaw) for c in out[:n.value]]
+
+    def matches(self) -> list[dict]:
+        """Every pair the last search aligned, with its ScanContext match, LM outcome, score and gate decision."""
+        n = C.c_int()
+        check(lib.lsd_galign_last_matches(self.h, None, 0, C.byref(n)))
+        out = (GalignMatch * max(n.value, 1))()
+        check(lib.lsd_galign_last_matches(self.h, out, n.value, C.byref(n)))
+        return [dict(new_slot=m.new_slot, ref_slot=m.ref_slot, sc_dist=m.sc_dist, sc_yaw=m.sc_yaw, converged=bool(m.converged),
+                     iterations=m.iterations, score=m.score, accepted=bool(m.accepted)) for m in out[:n.value]]
+
+    def set_max_batch_points(self, n: int):
+        """Memory budget of the following searches (sum over a batch of new-cloud points x neighbours); no effect on results."""
+        check(lib.lsd_galign_set_max_batch_points(self.h, int(n)))
+        self.params.max_batch_points = int(n)
+
+    def stats(self) -> dict:
+        """Work of the last search: kernel launches of the matching, host round trips (cost rounds), batches."""
+        ln, rd, nb = C.c_longlong(), C.c_int(), C.c_int()
+        check(lib.lsd_galign_last_stats(self.h, C.byref(ln), C.byref(rd), C.byref(nb)))
+        return dict(launches=ln.value, rounds=rd.value, batches=nb.value)
+
+    def match(self, new_slot: int, ref_slots, guesses, serial: bool = False) -> dict:
+        """FAST_VGICP of new_slot against each of ref_slots from guesses, batched or (serial) one pair at a time through
+        the single-pair kernels on the same tables (parity tap and baseline)."""
+        ref = _slots(ref_slots)
+        n = ref.size
+        G = np.ascontiguousarray(guesses, np.float64).reshape(n, 4, 4)
+        T = np.zeros((n, 4, 4)); cv = np.zeros(n, np.int32); it = np.zeros(n, np.int32); fit = np.zeros(n)
+        ln, rd = C.c_longlong(), C.c_int()
+        check(lib.lsd_galign_match(self.h, int(new_slot), _ptr(ref), _ptr(G), n, int(bool(serial)), _ptr(T), _ptr(cv), _ptr(it),
+                                   _ptr(fit), C.byref(ln), C.byref(rd)))
+        logs = []
+        for i in range(n):
+            m = C.c_int()
+            check(lib.lsd_galign_iteration_log(self.h, i, None, 0, C.byref(m)))
+            lg = np.zeros((max(m.value, 1), 4))
+            check(lib.lsd_galign_iteration_log(self.h, i, _ptr(lg), m.value, C.byref(m)))
+            logs.append(lg[:m.value])
+        return dict(final=T, converged=cv.astype(bool), iterations=it, fitness=fit, launches=ln.value, rounds=rd.value,
+                    iteration_logs=logs)
+
+    def cost(self, new_slot: int, ref_slot: int, T, update: bool = True, deriv: bool = True):
+        """One VGICP cost evaluation of the pair through the batched kernel: (err, H, b, n_corr), as Matcher.cost."""
+        T = np.ascontiguousarray(T, np.float64)
+        H, b = np.zeros((6, 6)), np.zeros(6)
+        e, nc = C.c_double(), C.c_int()
+        check(lib.lsd_galign_cost(self.h, int(new_slot), int(ref_slot), _ptr(T), int(update), _ptr(H) if deriv else None,
+                                  _ptr(b) if deriv else None, C.byref(e), C.byref(nc)))
+        return e.value, H, b, nc.value
+
+
+def galign_merge_candidates(cand_idx, cand_dist, cand_shift, n_cand, dist_thres: float = 0.30):
+    """global_alignment.hpp:215-227 on lsd_sc_query output ([n_off, 10] each, n_cand [n_off]): the matches below
+    dist_thres merged per database index (pure host).  Returns (idx [m], sc_dist float32 [m], sc_yaw float32 [m])."""
+    idx = np.ascontiguousarray(cand_idx, np.int32).reshape(-1, 10)
+    n_off = idx.shape[0]
+    dist = np.ascontiguousarray(cand_dist, np.float64).reshape(n_off, 10)
+    sh = np.ascontiguousarray(cand_shift, np.int32).reshape(n_off, 10)
+    nc = np.ascontiguousarray(n_cand, np.int32).reshape(n_off)
+    cap = max(n_off * 10, 1)
+    oi, od, oy = np.zeros(cap, np.int32), np.zeros(cap, np.float32), np.zeros(cap, np.float32)
+    n = C.c_int()
+    check(lib.lsd_galign_merge_candidates(_ptr(idx), _ptr(dist), _ptr(sh), _ptr(nc), n_off, float(dist_thres), _ptr(oi), _ptr(od),
+                                          _ptr(oy), cap, C.byref(n)))
+    return oi[:n.value].copy(), od[:n.value].copy(), oy[:n.value].copy()
 
 
 def eskf_update_table(state, P, HTH, HTh, n_eff, R=0.001, max_iterations=4, eps=0.001, literal=False, converge_log=None):

@@ -24,8 +24,9 @@ struct LoopCand {
   Pose34f lin, ev;       // NDT: linearisation / evaluation pose; fitness: ev is the pose
 };
 
-// The candidate a block belongs to (blk_off ascending): computed once per block.
-__device__ __forceinline__ int loop_cand_of_block(const LoopCand* __restrict__ cands, int n_cand) {
+// The candidate a block belongs to (blk_off ascending): computed once per block.  Cand: LoopCand here, GaCand in galign.cu.
+template <class Cand>
+__device__ __forceinline__ int loop_cand_of_block(const Cand* __restrict__ cands, int n_cand) {
   __shared__ int s_c;
   if (threadIdx.x == 0) {
     int lo = 0, hi = n_cand - 1;
@@ -126,6 +127,66 @@ __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_batch_kernel(MapVie
 }  // namespace lsd
 
 // ==================================================================== host side
+namespace lsd {
+
+// Host side of a batched launch (the loop detector's candidates here, the global aligner's pairs in galign.cu): the
+// descriptors, partial rows, per-candidate done counters and mapped result rows, grown to the largest batch seen so that a
+// round allocates nothing.  Result row 0 holds the sequence number the last candidate to finish publishes (loop_finalize),
+// row 1 + c the sums of candidate c.
+template <class Cand>
+struct BatchScratch {
+  Cand* d_cand = nullptr; Cand* h_cand = nullptr; int cand_cap = 0;
+  double* d_partials = nullptr; size_t part_cap = 0;     // rows of kNV doubles
+  unsigned* d_done = nullptr;                            // [0] candidates finished, [1 + c] blocks of candidate c finished; self-resetting
+  double *h_res = nullptr, *d_res = nullptr;             // mapped
+  long long seq = 0;
+
+  // room for n candidates and `rows` partial rows
+  lsd_status_t reserve(int n, size_t rows) {
+    if (n > cand_cap) {
+      cudaFree(d_cand); cudaFreeHost(h_cand); cudaFree(d_done); cudaFreeHost(h_res);
+      d_cand = nullptr; h_cand = nullptr; d_done = nullptr; h_res = nullptr; cand_cap = 0;
+      const int cap = std::max(n, 32);
+      LSD_CUDA(cudaMalloc((void**)&d_cand, cap * sizeof(Cand)));
+      LSD_CUDA(cudaHostAlloc((void**)&h_cand, cap * sizeof(Cand), cudaHostAllocDefault));
+      LSD_CUDA(cudaMalloc((void**)&d_done, (cap + 1) * sizeof(unsigned)));
+      LSD_CUDA(cudaMemset(d_done, 0, (cap + 1) * sizeof(unsigned)));
+      LSD_CUDA(cudaHostAlloc((void**)&h_res, (size_t)(cap + 1) * kNV * 8, cudaHostAllocMapped));
+      memset(h_res, 0, (size_t)(cap + 1) * kNV * 8);
+      LSD_CUDA(cudaHostGetDevicePointer((void**)&d_res, h_res, 0));
+      cand_cap = cap;
+    }
+    if (rows > part_cap) {
+      cudaFree(d_partials); d_partials = nullptr; part_cap = 0;
+      LSD_CUDA(cudaMalloc((void**)&d_partials, rows * kNV * 8));
+      part_cap = rows;
+    }
+    return LSD_OK;
+  }
+  // h_cand[0, n) to the device on st; *s = the sequence number the launch is to publish
+  lsd_status_t upload(int n, cudaStream_t st, double* s) {
+    LSD_CUDA(cudaMemcpyAsync(d_cand, h_cand, n * sizeof(Cand), cudaMemcpyHostToDevice, st));
+    *s = (double)(++seq);
+    return LSD_OK;
+  }
+  lsd_status_t wait(cudaStream_t st, double s) const { return wait_seq(h_res, st, s, 20.0); }
+  const double* row(int i) const { return h_res + (size_t)(1 + i) * kNV; }
+  void release() { cudaFree(d_cand); cudaFreeHost(h_cand); cudaFree(d_partials); cudaFree(d_done); cudaFreeHost(h_res); }
+};
+
+// A device buffer of at least n elements (contents not kept); true in *grown when it was reallocated.
+template <class T>
+static lsd_status_t grow_dev(T*& p, size_t& cap, size_t n, bool* grown = nullptr) {
+  if (grown) *grown = n > cap;
+  if (n <= cap) return LSD_OK;
+  cudaFree(p); p = nullptr; cap = 0;
+  LSD_CUDA(cudaMalloc((void**)&p, n * sizeof(T)));
+  cap = n;
+  return LSD_OK;
+}
+
+}  // namespace lsd
+
 struct lsd_loop {
   lsd_loop_params_t p{};
   int device = 0;
@@ -139,12 +200,8 @@ struct lsd_loop {
   std::vector<double> kf_accum;
   double last_edge = 0.0;    // last_edge_accum_distance (loop_detector.hpp:60,216)
   // batch scratch, grown to the largest candidate set seen
-  lsd::LoopCand* d_cand = nullptr; lsd::LoopCand* h_cand = nullptr; int cand_cap = 0;
+  lsd::BatchScratch<lsd::LoopCand> b;
   int* d_corr = nullptr; size_t corr_cap = 0;
-  double* d_partials = nullptr; size_t part_cap = 0;     // rows of kNV doubles
-  unsigned* d_done = nullptr;                            // [0] candidates finished, [1 + c] blocks of candidate c finished; self-resetting
-  double *h_res = nullptr, *d_res = nullptr;             // mapped: [0] sequence number, row 1 + c = candidate c
-  long long seq = 0;
   // last lsd_loop_match
   std::vector<lsd::LmState> lm;
   std::vector<double> fitness;
@@ -154,33 +211,11 @@ struct lsd_loop {
 namespace lsd {
 
 static lsd_status_t loop_reserve(lsd_loop* h, const std::vector<int>& ns, int n_off) {
-  const int n = (int)ns.size();
   size_t rows = 0, corr = 0;
   for (int v : ns) { rows += (size_t)std::max(reg_grid(v), warp_grid(v)); corr += (size_t)n_off * v; }
-  if (n > h->cand_cap) {
-    cudaFree(h->d_cand); cudaFreeHost(h->h_cand); cudaFree(h->d_done); cudaFreeHost(h->h_res);
-    h->d_cand = nullptr; h->h_cand = nullptr; h->d_done = nullptr; h->h_res = nullptr; h->cand_cap = 0;
-    const int cap = std::max(n, 32);
-    LSD_CUDA(cudaMalloc((void**)&h->d_cand, cap * sizeof(LoopCand)));
-    LSD_CUDA(cudaHostAlloc((void**)&h->h_cand, cap * sizeof(LoopCand), cudaHostAllocDefault));
-    LSD_CUDA(cudaMalloc((void**)&h->d_done, (cap + 1) * sizeof(unsigned)));
-    LSD_CUDA(cudaMemset(h->d_done, 0, (cap + 1) * sizeof(unsigned)));
-    LSD_CUDA(cudaHostAlloc((void**)&h->h_res, (size_t)(cap + 1) * kNV * 8, cudaHostAllocMapped));
-    memset(h->h_res, 0, (size_t)(cap + 1) * kNV * 8);
-    LSD_CUDA(cudaHostGetDevicePointer((void**)&h->d_res, h->h_res, 0));
-    h->cand_cap = cap;
-  }
-  if (rows > h->part_cap) {
-    cudaFree(h->d_partials); h->d_partials = nullptr; h->part_cap = 0;
-    LSD_CUDA(cudaMalloc((void**)&h->d_partials, rows * kNV * 8));
-    h->part_cap = rows;
-  }
-  if (corr > h->corr_cap) {
-    cudaFree(h->d_corr); h->d_corr = nullptr; h->corr_cap = 0;
-    LSD_CUDA(cudaMalloc((void**)&h->d_corr, corr * sizeof(int)));
-    h->corr_cap = corr;
-  }
-  return LSD_OK;
+  lsd_status_t s = h->b.reserve((int)ns.size(), rows);
+  if (s) return s;
+  return grow_dev(h->d_corr, h->corr_cap, corr);
 }
 
 // setInputTarget(new_keyframe->cloud) (:156): NDT map of the target, plus its exact-NN point map for the fitness scores.
@@ -212,7 +247,7 @@ static lsd_status_t loop_fitness(lsd_loop* h, const std::vector<int>& slots, con
   if (s) return s;
   int blocks = 0;
   for (int i = 0; i < n; i++) {
-    LoopCand& c = h->h_cand[i];
+    LoopCand& c = h->b.h_cand[i];
     memset(&c, 0, sizeof(c));
     c.src_off = (int)h->kf_off[slots[i]]; c.n = ns[i]; c.row = i;
     c.warp_shape = ns[i] < kThreadShapeMin;
@@ -221,17 +256,18 @@ static lsd_status_t loop_fitness(lsd_loop* h, const std::vector<int>& slots, con
     c.ev = poses[i]; c.lin = poses[i];
   }
   cudaStream_t st = r->stream;
-  LSD_CUDA(cudaMemcpyAsync(h->d_cand, h->h_cand, n * sizeof(LoopCand), cudaMemcpyHostToDevice, st));
-  const double seq = (double)(++h->seq);
+  double seq = 0;
+  s = h->b.upload(n, st, &seq);
+  if (s) return s;
   const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
-  fitness_batch_kernel<<<blocks, kRegWarps * 32, 0, st>>>(r->tgt_map->view, h->d_pool, h->d_cand, n, search_sq, (float)max_range,
-                                                         exact ? r->d_tgt : nullptr, r->n_tgt, h->d_partials, h->d_done, h->d_res, seq);
+  fitness_batch_kernel<<<blocks, kRegWarps * 32, 0, st>>>(r->tgt_map->view, h->d_pool, h->b.d_cand, n, search_sq, (float)max_range,
+                                                         exact ? r->d_tgt : nullptr, r->n_tgt, h->b.d_partials, h->b.d_done, h->b.d_res, seq);
   LSD_CUDA(cudaGetLastError());
   (*launches)++;
-  s = wait_seq(h->h_res, st, seq, 20.0);
+  s = h->b.wait(st, seq);
   if (s) return s;
   for (int i = 0; i < n; i++) {
-    const double sum = h->h_res[(size_t)(1 + i) * kNV], cnt = h->h_res[(size_t)(1 + i) * kNV + 1];
+    const double sum = h->b.row(i)[0], cnt = h->b.row(i)[1];
     score[i] = cnt > 0 ? sum / cnt : DBL_MAX;
     if (count) count[i] = cnt;
   }
@@ -261,7 +297,7 @@ static lsd_status_t loop_coarse(lsd_loop* h, int target, const int32_t* cand, co
     for (int i = 0; i < n; i++) {
       const LmState& m = h->lm[i];
       if (m.done) continue;
-      LoopCand& c = h->h_cand[na++];
+      LoopCand& c = h->b.h_cand[na++];
       memset(&c, 0, sizeof(c));
       c.src_off = (int)h->kf_off[cand[i]]; c.n = ns[i]; c.row = i;
       c.n_blk = reg_grid(ns[i]); c.blk_off = blocks; blocks += c.n_blk;
@@ -271,17 +307,19 @@ static lsd_status_t loop_coarse(lsd_loop* h, int target, const int32_t* cand, co
       c.lin = c.ev;   // read only when update (the linearisation pose is the evaluation pose then)
     }
     if (na == 0) break;
-    LSD_CUDA(cudaMemcpyAsync(h->d_cand, h->h_cand, na * sizeof(LoopCand), cudaMemcpyHostToDevice, st));
-    const double seq = (double)(++h->seq);
-    ndt_cost_batch_kernel<<<blocks, 256, 0, st>>>(r->ndt, h->d_pool, h->d_cand, na, n_off, h->d_corr, h->d_partials, h->d_done, h->d_res, seq);
+    double seq = 0;
+    s = h->b.upload(na, st, &seq);
+    if (s) return s;
+    ndt_cost_batch_kernel<<<blocks, 256, 0, st>>>(r->ndt, h->d_pool, h->b.d_cand, na, n_off, h->d_corr, h->b.d_partials, h->b.d_done,
+                                                  h->b.d_res, seq);
     LSD_CUDA(cudaGetLastError());
     (*launches)++; (*rounds)++;
-    s = wait_seq(h->h_res, st, seq, 20.0);
+    s = h->b.wait(st, seq);
     if (s) return s;
     for (int i = 0; i < n; i++) {
       LmState& m = h->lm[i];
       if (m.done) continue;
-      const double* res = h->h_res + (size_t)(1 + i) * kNV;
+      const double* res = h->b.row(i);
       double H[36], b[6];
       if (m.want_update) unpack_hb(res, H, b);
       lm_feed(m, H, b, res[27]);
@@ -417,8 +455,8 @@ lsd_status_t lsd_loop_create(lsd_loop_t** out, const lsd_loop_params_t* p) {
 lsd_status_t lsd_loop_destroy(lsd_loop_t* h) {
   if (!h) return LSD_OK;
   if (h->ndt) { cudaSetDevice(h->ndt->device); cudaStreamSynchronize(h->ndt->stream); }
-  cudaFree(h->d_pool); cudaFree(h->d_cand); cudaFreeHost(h->h_cand); cudaFree(h->d_corr); cudaFree(h->d_partials);
-  cudaFree(h->d_done); cudaFreeHost(h->h_res);
+  cudaFree(h->d_pool); cudaFree(h->d_corr);
+  h->b.release();
   lsd_reg_destroy(h->ndt);
   lsd_reg_destroy(h->gicp);
   delete h;

@@ -527,6 +527,58 @@ __global__ void __launch_bounds__(256) vgicp_finalize_kernel(const NdtBuildLine*
   out[s] = o;
 }
 
+// One source point of a VGICP cost evaluation: update_correspondences at T with the Mahalanobis matrices stored (update)
+// or reused, then linearize / compute_error (fast_vgicp_impl.hpp:72-207), double.  `corr` / `maha` point at the [n_off, n]
+// correspondence slots / 6 [n_off, n] doubles of this cloud.  Shared by the single-pair kernel below (compile-time flags)
+// and the batched global-alignment kernel (galign.cu, flags per candidate): the same expressions, so the same bits.
+__device__ __forceinline__ void vgicp_point(const VgView& v, const float4 a, const double* __restrict__ src_nrm, int i, int n, int n_off,
+                                            const Pose34d& T, int* __restrict__ corr, double* __restrict__ maha, bool update,
+                                            bool deriv, double (&vals)[29]) {
+  const double3 t = xform(T, a);
+  int3 c = make_int3(0, 0, 0);
+  double rn[3] = {0.0, 0.0, 0.0};
+  if (update) {
+    c = vg_coord(t.x, t.y, t.z, v.res);
+    const double* na = src_nrm + 4 * (size_t)i;
+    rn[0] = T.R[0] * na[0] + T.R[1] * na[1] + T.R[2] * na[2];
+    rn[1] = T.R[3] * na[0] + T.R[4] * na[1] + T.R[5] * na[2];
+    rn[2] = T.R[6] * na[0] + T.R[7] * na[1] + T.R[8] * na[2];
+  }
+#pragma unroll 1
+  for (int o = 0; o < n_off; o++) {
+    const size_t q = (size_t)o * n + i;
+    int slot;
+    if (update) {
+      const int3 d = stencil_offset(o, n_off);
+      slot = voxel_lookup(v, c.x + d.x, c.y + d.y, c.z + d.z);
+      corr[q] = slot;
+    } else {
+      slot = corr[q];
+    }
+    if (slot < 0) continue;
+    vals[28] += 1.0;
+    const VgLine* ln = v.lines + slot;
+    double M[3][3];
+    if (update) {
+      // RCR = cov_B + R cov_A R^T with cov_A = I - 0.999 n n^T
+      const double A0 = ln->cov[0] + 1.0 - 0.999 * rn[0] * rn[0], A1 = ln->cov[1] - 0.999 * rn[0] * rn[1], A2 = ln->cov[2] - 0.999 * rn[0] * rn[2];
+      const double A4 = ln->cov[3] + 1.0 - 0.999 * rn[1] * rn[1], A5 = ln->cov[4] - 0.999 * rn[1] * rn[2], A8 = ln->cov[5] + 1.0 - 0.999 * rn[2] * rn[2];
+      const double c00 = A4 * A8 - A5 * A5, c01 = A5 * A2 - A1 * A8, c02 = A1 * A5 - A4 * A2;
+      const double idet = 1.0 / (A0 * c00 + A1 * c01 + A2 * c02);
+      M[0][0] = c00 * idet; M[0][1] = c01 * idet; M[0][2] = c02 * idet;
+      M[1][1] = (A0 * A8 - A2 * A2) * idet; M[1][2] = (A2 * A1 - A0 * A5) * idet; M[2][2] = (A0 * A4 - A1 * A1) * idet;
+      M[1][0] = M[0][1]; M[2][0] = M[0][2]; M[2][1] = M[1][2];
+      double* Ms = maha + 6 * q;
+      Ms[0] = M[0][0]; Ms[1] = M[0][1]; Ms[2] = M[0][2]; Ms[3] = M[1][1]; Ms[4] = M[1][2]; Ms[5] = M[2][2];
+    } else {
+      const double* Ms = maha + 6 * q;
+      M[0][0] = Ms[0]; M[0][1] = M[1][0] = Ms[1]; M[0][2] = M[2][0] = Ms[2]; M[1][1] = Ms[3]; M[1][2] = M[2][1] = Ms[4]; M[2][2] = Ms[5];
+    }
+    const double w = sqrt((double)ln->n);
+    accum_d2d(vals, M, make_double3(ln->mean[0] - t.x, ln->mean[1] - t.y, ln->mean[2] - t.z), t, w, deriv);
+  }
+}
+
 // linearize (UPDATE: update_correspondences at T, Mahalanobis matrices stored) / compute_error (reuse).
 // One thread per source point, double.
 template <bool UPDATE, bool DERIV>
@@ -539,51 +591,8 @@ __global__ void __launch_bounds__(256) vgicp_cost_kernel(VgView v, const float4*
 #pragma unroll
   for (int j = 0; j < 29; j++) vals[j] = 0.0;
 #pragma unroll 1
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double3 t = xform(T, __ldg(src + i));
-    int3 c = make_int3(0, 0, 0);
-    double rn[3] = {0.0, 0.0, 0.0};
-    if (UPDATE) {
-      c = vg_coord(t.x, t.y, t.z, v.res);
-      const double* na = src_nrm + 4 * (size_t)i;
-      rn[0] = T.R[0] * na[0] + T.R[1] * na[1] + T.R[2] * na[2];
-      rn[1] = T.R[3] * na[0] + T.R[4] * na[1] + T.R[5] * na[2];
-      rn[2] = T.R[6] * na[0] + T.R[7] * na[1] + T.R[8] * na[2];
-    }
-#pragma unroll 1
-    for (int o = 0; o < n_off; o++) {
-      const size_t q = (size_t)o * n + i;
-      int slot;
-      if (UPDATE) {
-        const int3 d = stencil_offset(o, n_off);
-        slot = voxel_lookup(v, c.x + d.x, c.y + d.y, c.z + d.z);
-        corr[q] = slot;
-      } else {
-        slot = corr[q];
-      }
-      if (slot < 0) continue;
-      vals[28] += 1.0;
-      const VgLine* ln = v.lines + slot;
-      double M[3][3];
-      if (UPDATE) {
-        // RCR = cov_B + R cov_A R^T with cov_A = I - 0.999 n n^T
-        const double A0 = ln->cov[0] + 1.0 - 0.999 * rn[0] * rn[0], A1 = ln->cov[1] - 0.999 * rn[0] * rn[1], A2 = ln->cov[2] - 0.999 * rn[0] * rn[2];
-        const double A4 = ln->cov[3] + 1.0 - 0.999 * rn[1] * rn[1], A5 = ln->cov[4] - 0.999 * rn[1] * rn[2], A8 = ln->cov[5] + 1.0 - 0.999 * rn[2] * rn[2];
-        const double c00 = A4 * A8 - A5 * A5, c01 = A5 * A2 - A1 * A8, c02 = A1 * A5 - A4 * A2;
-        const double idet = 1.0 / (A0 * c00 + A1 * c01 + A2 * c02);
-        M[0][0] = c00 * idet; M[0][1] = c01 * idet; M[0][2] = c02 * idet;
-        M[1][1] = (A0 * A8 - A2 * A2) * idet; M[1][2] = (A2 * A1 - A0 * A5) * idet; M[2][2] = (A0 * A4 - A1 * A1) * idet;
-        M[1][0] = M[0][1]; M[2][0] = M[0][2]; M[2][1] = M[1][2];
-        double* Ms = maha + 6 * q;
-        Ms[0] = M[0][0]; Ms[1] = M[0][1]; Ms[2] = M[0][2]; Ms[3] = M[1][1]; Ms[4] = M[1][2]; Ms[5] = M[2][2];
-      } else {
-        const double* Ms = maha + 6 * q;
-        M[0][0] = Ms[0]; M[0][1] = M[1][0] = Ms[1]; M[0][2] = M[2][0] = Ms[2]; M[1][1] = Ms[3]; M[1][2] = M[2][1] = Ms[4]; M[2][2] = Ms[5];
-      }
-      const double w = sqrt((double)ln->n);
-      accum_d2d(vals, M, make_double3(ln->mean[0] - t.x, ln->mean[1] - t.y, ln->mean[2] - t.z), t, w, DERIV);
-    }
-  }
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    vgicp_point(v, __ldg(src + i), src_nrm, i, n, n_off, T, corr, maha, UPDATE, DERIV, vals);
   block_partials<29>(vals, partials);
   grid_finalize<29>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
@@ -1222,6 +1231,34 @@ static lsd_status_t build_point_map(lsd_reg* r, lsd_map** mp, const float4* d_pt
 
 static void detach_map_stream(lsd_map* m) { if (m) m->stream = nullptr; }
 
+// calculate_covariances (fast_gicp_impl.hpp:244-303) of the cloud d_pts: its exact-NN point map built into *mp, then the
+// k-NN covariance of every point as its smallest-eigenvalue direction and neighbour count in nrm [n, 4], on the handle's
+// stream.  GICP / VGICP sources and targets of lsd_reg, and the key frames of the global aligner (galign.cu).
+static lsd_status_t gicp_covariances(lsd_reg* r, lsd_map** mp, const float4* d_pts, int n, double* nrm) {
+  lsd_status_t s = build_point_map(r, mp, d_pts, n);
+  if (s) return s;
+  cudaStream_t st = r->stream;
+  gicp_normals_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>((*mp)->view, d_pts, n, r->p.k_correspondences, (float)r->p.normal_search_sq, nrm);
+  gicp_normals_complete_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>(d_pts, n, r->p.k_correspondences, nrm);
+  LSD_CUDA(cudaGetLastError());
+  r->launches += 3;
+  return LSD_OK;
+}
+
+// GaussianVoxelMap::create_voxelmap (built lazily by the reference, fast_vgicp_impl.hpp:121-124) of the target d_pts with
+// its covariances nrm into vg (lines reallocated when the size changes), at the handle's resolution.
+static lsd_status_t vgicp_voxel_table(lsd_reg* r, const float4* d_pts, const double* nrm, int n, VgView& vg, unsigned long long& vg_lines) {
+  cudaStream_t st = r->stream;
+  vg.res = r->p.resolution;
+  return build_voxel_table(r, n, "VGICP", vg, vg_lines,
+      [&](NdtBuildLine* build, unsigned long long mask, unsigned* d_fail) {
+        vgicp_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, mask, vg.res, d_pts, nrm, n, d_fail);
+      },
+      [&](const NdtBuildLine* build, unsigned long long lines, unsigned* d_vox) {
+        vgicp_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, vg.lines, lines, d_vox);
+      });
+}
+
 // setInputTarget: NDT builds the Gaussian voxel map immediately (ndt_cuda.cu:105-114); GICP indexes the
 // cloud and computes its covariances (fast_gicp_impl.hpp:112-114).
 lsd_status_t lsd_reg_set_target_dev(lsd_reg_t* r, const float* pts_dev, int n) {
@@ -1248,23 +1285,11 @@ lsd_status_t lsd_reg_set_target_dev(lsd_reg_t* r, const float* pts_dev, int n) {
         });
     if (s) return s;
   } else {
-    lsd_status_t s = build_point_map(r, &r->tgt_map, r->d_tgt, n);
+    lsd_status_t s = gicp_covariances(r, &r->tgt_map, r->d_tgt, n, r->d_tgt_nrm);
     if (s) return s;
-    gicp_normals_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_tgt, n, r->p.k_correspondences,
-                                                                (float)r->p.normal_search_sq, r->d_tgt_nrm);
-    gicp_normals_complete_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>(r->d_tgt, n, r->p.k_correspondences, r->d_tgt_nrm);
-    LSD_CUDA(cudaGetLastError());
-    r->launches += 3;
     r->tgt_map_built = true;
-    if (r->p.kind == LSD_REG_VGICP) {  // GaussianVoxelMap::create_voxelmap (built lazily by the reference, fast_vgicp_impl.hpp:121-124)
-      r->vg.res = r->p.resolution;
-      s = build_voxel_table(r, n, "VGICP", r->vg, r->vg_lines,
-          [&](NdtBuildLine* build, unsigned long long mask, unsigned* d_fail) {
-            vgicp_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, mask, r->vg.res, r->d_tgt, r->d_tgt_nrm, n, d_fail);
-          },
-          [&](const NdtBuildLine* build, unsigned long long lines, unsigned* d_vox) {
-            vgicp_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, r->vg.lines, lines, d_vox);
-          });
+    if (r->p.kind == LSD_REG_VGICP) {
+      s = vgicp_voxel_table(r, r->d_tgt, r->d_tgt_nrm, n, r->vg, r->vg_lines);
       if (s) return s;
     }
     LSD_CUDA(cudaStreamSynchronize(st));
@@ -1281,13 +1306,8 @@ lsd_status_t lsd_reg_set_source_dev(lsd_reg_t* r, const float* pts_dev, int n) {
   LSD_CUDA(cudaMemcpyAsync(r->d_src, pts_dev, (size_t)n * 16, cudaMemcpyDeviceToDevice, st));
   r->n_src = n;
   if (r->p.kind != LSD_REG_NDT_P2D) {  // source covariances (fast_gicp_impl.hpp:109-111)
-    s = build_point_map(r, &r->src_map, r->d_src, n);
+    s = gicp_covariances(r, &r->src_map, r->d_src, n, r->d_src_nrm);
     if (s) return s;
-    gicp_normals_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>(r->src_map->view, r->d_src, n, r->p.k_correspondences,
-                                                                (float)r->p.normal_search_sq, r->d_src_nrm);
-    gicp_normals_complete_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>(r->d_src, n, r->p.k_correspondences, r->d_src_nrm);
-    LSD_CUDA(cudaGetLastError());
-    r->launches += 3;
     LSD_CUDA(cudaStreamSynchronize(st));
   }
   return LSD_OK;

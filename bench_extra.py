@@ -5,6 +5,7 @@
   config[4]  detection voxelizer: 200 k pts, 4-frame window
   loop       loop-closure detection: one new key frame vs C candidates (C = 4, 16, 32), ~30 k pts each
   galign     global-alignment closure search: 72 reference x 100 new key frames, ~13 k pts each, hundreds of pairs
+  floor      floor detection, mapping preset, on ~100 k-return scans (device and host input)
 Prints one JSON object per config with device times (CUDA events via torch on the default stream are
 NOT used: the library runs on its own stream, so wall time around synchronous C-ABI calls is reported)
 and the CPU restatement timed on a bounded sample.
@@ -472,6 +473,74 @@ def galign(args):
     print(json.dumps(out))
 
 
+def floor(args):
+    """Floor detection, LSD_FLOOR_MAPPING preset (VoxelGrid 0.2 + distance filter, clip, k = 10 normal filter, RANSAC) on
+    BASELINE config[1]-size scans (~100 k returns, sensor 1.8 m above the ground), device-resident and host input.  Device
+    kernel time by stage from torch.profiler; the CPU restatement (tests/floor_oracle.py, numpy + scipy) timed by stage,
+    labelled as the restatement: PCL itself cannot be built here."""
+    import torch
+    import lsdreg
+    from lsdreg import synth
+    card = _card()
+    scans = [synth.scan64(500 + i, 1563, synth.rot_from_rpy(0.0, 0.0, 0.4 * i), synth.block_center(0, 0) + np.array([1.5 * i - 3.0, -2.0, 0.0]))
+             for i in range(args.floor_scans)]
+    det = lsdreg.FloorDetector(lsdreg.FLOOR_MAPPING)
+    dev = [torch.from_numpy(s).cuda() for s in scans]
+    torch.cuda.synchronize()
+    for s in dev:
+        det.detect(s)                                   # warm-up: buffers sized
+    out = dict(config="floor detection, mapping preset: %d scans x ~%d returns" % (len(scans), int(np.mean([s.shape[0] for s in scans]))), **card)
+    for label, inputs in (("device_input", dev), ("host_input", scans)):
+        ms, res = [], []
+        for _ in range(args.floor_reps):
+            for s in inputs:
+                t0 = time.perf_counter()
+                r = det.detect(s)
+                ms.append((time.perf_counter() - t0) * 1e3)
+                res.append(r)
+        out[label] = dict(frames=len(ms), ms_median=float(np.median(ms)), ms_p95=float(np.percentile(ms, 95)),
+                          launches_median=float(np.median([r["launches"] for r in res])),
+                          round_trips_median=float(np.median([r["round_trips"] for r in res])),
+                          hypotheses_scored_median=float(np.median([r["hypotheses_scored"] for r in res])),
+                          iterations_median=float(np.median([r["iterations"] for r in res])),
+                          found=int(sum(r["found"] for r in res)),
+                          candidates_median=float(np.median([r["n_candidates"] for r in res])),
+                          prefiltered_median=float(np.median([r["n_prefiltered"] for r in res])))
+    try:   # device time by stage: kernel durations grouped by kernel name
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for s in dev:
+                det.detect(s)
+        stage_of = lambda n: ("voxelgrid" if n.startswith("vg_") or "vg_" in n else "clip+insert" if "floor_clip" in n  # noqa: E731
+                              else "normals" if "normals" in n or "complete" in n else "ransac" if "sample" in n or "score" in n
+                              else "compaction" if "compact" in n else "other")
+        by = {}
+        for e in prof.events():
+            if getattr(e, "device_type", None) is not None and str(e.device_type).endswith("CUDA") and ("kernel" in str(getattr(e, "name", "")).lower() or "lsd" in e.name):
+                by[stage_of(e.name)] = by.get(stage_of(e.name), 0.0) + e.device_time_total / 1e3
+        out["device_kernel_ms_per_frame_by_stage"] = {k: v / len(dev) for k, v in sorted(by.items())}
+    except Exception as e:  # the profiler must never take the measurement down
+        out["device_kernel_ms_per_frame_by_stage"] = dict(error=repr(e)[:200])
+    if not args.no_cpu:
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        import floor_oracle as FO
+        p = FO.default_params(FO.MAPPING)
+        st = {"prefilter": [], "clip": [], "normals": [], "ransac": []}
+        for s in scans:
+            t0 = time.perf_counter(); pre = FO.prefilter(s, p)
+            t1 = time.perf_counter(); cl = pre[FO.clip_mask(pre, p)]
+            t2 = time.perf_counter(); nrm, _, _ = FO.normals(cl[:, :3]); cand = cl[np.abs(FO.normal_nz(nrm)).astype(np.float64) > np.cos(np.pi / 9)]
+            t3 = time.perf_counter(); FO.ransac(cand, p["ransac_threshold"]) if cand.shape[0] >= p["floor_pts_thresh"] else None
+            t4 = time.perf_counter()
+            for k, a, b in (("prefilter", t0, t1), ("clip", t1, t2), ("normals", t2, t3), ("ransac", t3, t4)):
+                st[k].append((b - a) * 1e3)
+        out["restatement_cpu_ms_median_by_stage"] = {k: float(np.median(v)) for k, v in st.items()}
+        out["restatement_cpu_ms_median"] = float(np.median(np.sum([st[k] for k in st], axis=0)))
+        out["restatement_note"] = "numpy/scipy restatement of the PCL rules (single process), not PCL"
+    det.close()
+    print(json.dumps(out))
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="ndt,gicp,vfe")
@@ -487,6 +556,8 @@ if __name__ == "__main__":
     ap.add_argument("--galign-reps", type=int, default=3)
     ap.add_argument("--galign-ref-pairs", type=int, default=24)
     ap.add_argument("--galign-ref-threads", type=int, default=4, help="FastVGICP threads (setNumThreads(4), registrations.cpp:59)")
+    ap.add_argument("--floor-scans", type=int, default=8)
+    ap.add_argument("--floor-reps", type=int, default=5)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-ref-cuda", action="store_true", help="skip the legs that time the reference's own CUDA NDT / VGICP (oracle/_ref/libref_cuda*.so)")
     a = ap.parse_args()
@@ -498,6 +569,6 @@ if __name__ == "__main__":
         with contextlib.redirect_stdout(buf):
             lsdreg.init(int(os.environ.get("LOCAL_RANK", 0)))
             for w in a.which.split(","):
-                {"ndt": ndt, "gicp": gicp, "vfe": vfe, "loop": loop, "galign": galign}[w](a)
+                {"ndt": ndt, "gicp": gicp, "vfe": vfe, "loop": loop, "galign": galign, "floor": floor}[w](a)
     sys.stdout.write(buf.getvalue())
     sys.stdout.flush()

@@ -760,6 +760,84 @@ lsd_status_t lsd_sc_distance(lsd_sc_t* s, const double* desc_a_host, const doubl
 lsd_status_t lsd_sc_detect_closest(lsd_sc_t* s, int slot, double dist_thres, int32_t* loop_id, float* yaw_rad, double* score);
 lsd_status_t lsd_sc_detect_candidates(lsd_sc_t* s, int slot, double dist_thres, int32_t* idx10, float* yaw10, float* dist10, int32_t* n);
 
+/* ------------------------------------------------------------------------------------------
+ * Floor detection — replaces FloorDetectionNodelet::detect (slam/backend/hdl_graph_slam/apps/floor_detection_nodelet.cpp:79-193)
+ * after PrefilteringNodelet (prefiltering_nodelet.cpp:91-165), the per-frame work of FastLIO's "FLIO Floor" thread
+ * (slam/mapping/fastlio/src/fastlio.cpp:279-292), and the two detect_ground copies (slam/src/graph_utils.cpp:329-382,
+ * slam/localization/map_render/map_render.cpp:81-134).  One call = one frame on the handle's own stream: VoxelGrid + distance
+ * filter (optional), the two PlaneClipper3D height clips, NormalEstimation (k = 10) + the |n_z| filter, and
+ * RandomSampleConsensus with SampleConsensusModelPlane (PCL 1.9.1, boost::mt19937 seeded 12345 on every call, so the floor
+ * is a pure function of the cloud).  The rules are restated in DESIGN.md section 5f.  A handle is confined to one host
+ * thread at a time; handles on different threads (and an lsd_lio_t / lsd_fastlio_t) run side by side.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct lsd_floor lsd_floor_t;
+#define LSD_FLOOR_MAPPING 0   /* prefiltering_nodelet + FloorDetectionNodelet: leaf 0.2, 0.1 < d < 100, clip 2.0 / -1.0      */
+#define LSD_FLOOR_GROUND 1    /* graph_utils.cpp::detect_ground: no prefilter, clip 1.5 / -1.5, threshold 0.1, inlier cloud    */
+#define LSD_FLOOR_RENDER 2    /* map_render.cpp::detect_ground: as GROUND with a RANSAC threshold of 0.2                      */
+typedef struct lsd_floor_params {
+  float prefilter_leaf;             /* VoxelGrid leaf of the prefilter (0 = no prefilter, and no distance filter)             */
+  double distance_near, distance_far; /* distance filter d > near && d < far, d = double(float |xyz|) (:152-155)             */
+  float clip_keep_d;                /* keep z >= -clip_keep_d (plane (0, 0, 1, d), ExtractIndices negative = false)          */
+  float clip_cut_d;                 /* then drop z >= -clip_cut_d (ExtractIndices negative = true)                           */
+  int use_normal_filtering;         /* 1 (floor_detection_nodelet.cpp:44)                                                   */
+  int normal_k;                     /* 10 (setKSearch(10)); no other value is supported                                     */
+  double normal_filter_deg;         /* keep |n_z| > cos(20 deg)                                                             */
+  float viewpoint_z;                /* setViewPoint(0, 0, sensor_height = 0): the sign of the normals only                  */
+  double ransac_threshold;          /* setDistanceThreshold: 0.1 (0.2 for RENDER)                                           */
+  double ransac_probability;        /* 0.99, SampleConsensus default                                                        */
+  int ransac_max_iterations;        /* 10000, SampleConsensus default                                                       */
+  int floor_pts_thresh;             /* 1024: fewer candidates or inliers = no floor                                         */
+  double floor_normal_deg;          /* 10: |c2| < cos(10 deg) = not vertical                                                */
+  int hypotheses_per_batch;         /* hypotheses drawn and scored per launch pair (256, 1 .. 12288); no output depends on it */
+} lsd_floor_params_t;
+
+#define LSD_FLOOR_FOUND 0
+#define LSD_FLOOR_EMPTY 1             /* the input cloud is empty                                                            */
+#define LSD_FLOOR_FEW_CANDIDATES 2    /* fewer than floor_pts_thresh points after the clip and the normal filter (:91-93)    */
+#define LSD_FLOOR_NO_MODEL 3          /* RANSAC found no model (no sample could be drawn, or fewer than 3 candidates)       */
+#define LSD_FLOOR_FEW_INLIERS 4       /* fewer than floor_pts_thresh inliers (:105-107)                                      */
+#define LSD_FLOOR_NOT_VERTICAL 5      /* |c2| < cos(floor_normal_deg) (:115-119)                                             */
+typedef struct lsd_floor_result {
+  int32_t found, reason;            /* reason: LSD_FLOOR_*                                                                   */
+  float coeffs[4];                  /* the plane, c2 >= 0 when found (:122-124); RANSAC's best model otherwise              */
+  int32_t n_input, n_prefiltered, n_clipped, n_candidates, n_inliers;
+  int32_t map_dropped;              /* points the normals' point map refused: every point then took the exact scan        */
+  int32_t iterations, skipped;      /* RandomSampleConsensus's iterations_ and skipped_count at the stop                   */
+  int32_t best_hypothesis;          /* draw-order index of the best model (-1: none)                                       */
+  int32_t batches;                  /* sampler + scoring launch pairs                                                      */
+  int64_t hypotheses_scored;        /* batches x hypotheses_per_batch                                                      */
+  int32_t launches, round_trips;    /* kernel launches and host waits of the call                                         */
+} lsd_floor_result_t;
+
+#define LSD_FLOOR_STAGE_PREFILTERED 0
+#define LSD_FLOOR_STAGE_CLIPPED 1
+#define LSD_FLOOR_STAGE_CANDIDATES 2
+#define LSD_FLOOR_STAGE_INLIERS 3
+
+void lsd_floor_default_params(lsd_floor_params_t* p, int preset);
+lsd_status_t lsd_floor_create(lsd_floor_t** out, const lsd_floor_params_t* p);
+lsd_status_t lsd_floor_destroy(lsd_floor_t* f);
+/* One frame ([n,4] xyzi, sensor frame).  The device entry reads xyzi_dev on the handle's stream. */
+lsd_status_t lsd_floor_detect(lsd_floor_t* f, const float* xyzi_host, int n, lsd_floor_result_t* res);
+lsd_status_t lsd_floor_detect_dev(lsd_floor_t* f, const float* xyzi_dev, int n, lsd_floor_result_t* res);
+/* The cloud of a stage of the last call (LSD_FLOOR_STAGE_*), in order; INLIERS is detect_ground's output cloud.
+ * Writes up to cap points; *n = the stage's size.  The _dev form returns a device pointer valid until the next detect. */
+lsd_status_t lsd_floor_get_cloud(lsd_floor_t* f, int stage, float* out, int cap, int* n);
+lsd_status_t lsd_floor_get_cloud_dev(lsd_floor_t* f, int stage, const float** xyzi_dev, int* n);
+/* Per clipped point of the last call: the normal and curvature (nx, ny, nz, curvature) after flipNormalTowardsViewpoint,
+ * and the fp32 covariance (xx, xy, xz, yy, yz, zz) of its 10 neighbours.  NaN for fewer than 3 neighbours.  Either output
+ * may be NULL; *n = clipped points (0 without normal filtering). */
+lsd_status_t lsd_floor_get_normals(lsd_floor_t* f, float* normal4, float* cov6, int cap, int* n);
+/* The hypotheses RANSAC drew in the last call, in draw order, up to the stop: candidate indices [n,3], flag (1 model,
+ * 0 collinear = skipped, -1 no sample could be drawn) and inlier count.  Any output may be NULL. */
+lsd_status_t lsd_floor_last_samples(lsd_floor_t* f, int32_t* idx3, int32_t* flags, int32_t* counts, int cap, int* n);
+/* The stop rule of RandomSampleConsensus::computeModel, pure host (works without a device), on hypotheses in draw order
+ * (inlier counts and flags as lsd_floor_last_samples gives them) over a cloud of n_points: *consumed = hypotheses drawn
+ * before the loop ended (-1: it had not ended after n), *best = index of the best model (-1: none), *iterations /
+ * *skipped = iterations_ / skipped_count (either may be NULL). */
+lsd_status_t lsd_ransac_replay(const int32_t* counts, const int32_t* flags, int n, int n_points, double probability,
+                               int max_iterations, int* consumed, int* best, int* iterations, int* skipped);
+
 /* Host-side manifold helpers (exported so bindings/tests use the same algebra as the filter).
  * IMU_Processing.hpp:224-230 initial covariance; state_ikfom boxplus/boxminus. */
 void lsd_lio_init_cov(double* P529);

@@ -99,6 +99,26 @@ class VfeParams(C.Structure):
                 ("max_points_per_voxel", C.c_int), ("max_voxels", C.c_int), ("max_points", C.c_int), ("num_feature", C.c_int),
                 ("max_frame_num", C.c_int), ("unordered_ids", C.c_int)]
 
+class FloorParams(C.Structure):
+    _fields_ = [("prefilter_leaf", C.c_float), ("distance_near", C.c_double), ("distance_far", C.c_double),
+                ("clip_keep_d", C.c_float), ("clip_cut_d", C.c_float), ("use_normal_filtering", C.c_int), ("normal_k", C.c_int),
+                ("normal_filter_deg", C.c_double), ("viewpoint_z", C.c_float), ("ransac_threshold", C.c_double),
+                ("ransac_probability", C.c_double), ("ransac_max_iterations", C.c_int), ("floor_pts_thresh", C.c_int),
+                ("floor_normal_deg", C.c_double), ("hypotheses_per_batch", C.c_int)]
+
+
+class FloorResult(C.Structure):
+    _fields_ = [("found", C.c_int32), ("reason", C.c_int32), ("coeffs", C.c_float * 4), ("n_input", C.c_int32),
+                ("n_prefiltered", C.c_int32), ("n_clipped", C.c_int32), ("n_candidates", C.c_int32), ("n_inliers", C.c_int32),
+                ("map_dropped", C.c_int32), ("iterations", C.c_int32), ("skipped", C.c_int32), ("best_hypothesis", C.c_int32),
+                ("batches", C.c_int32), ("hypotheses_scored", C.c_int64), ("launches", C.c_int32), ("round_trips", C.c_int32)]
+
+
+# lsd_floor_default_params presets, FloorResult.reason and the stages of FloorDetector.cloud (LSD_FLOOR_*)
+FLOOR_MAPPING, FLOOR_GROUND, FLOOR_RENDER = range(3)
+FLOOR_FOUND, FLOOR_EMPTY, FLOOR_FEW_CANDIDATES, FLOOR_NO_MODEL, FLOOR_FEW_INLIERS, FLOOR_NOT_VERTICAL = range(6)
+FLOOR_STAGES = {"prefiltered": 0, "clipped": 1, "candidates": 2, "inliers": 3}
+
 # every symbol include/lsdreg.h declares: (name, restype, argtypes)
 _vp, _i, _f, _d = C.c_void_p, C.c_int, C.c_float, C.c_double
 _pp = C.POINTER(C.c_void_p)
@@ -261,6 +281,16 @@ SIGNATURES = [
     ("lsd_keyframe_filter_dev", _i, [_vp, _i, _f, _i, _f, _f, _vp, _pi]),
     ("lsd_keyframe_save", _i, [C.c_char_p, C.c_uint64, C.c_int64, _vp, _i, _vp]),
     ("lsd_keyframe_load", _i, [C.c_char_p, _pu64, C.POINTER(C.c_int64), _vp, _vp, _i, _pi]),
+    ("lsd_floor_default_params", None, [C.POINTER(FloorParams), _i]),
+    ("lsd_floor_create", _i, [_pp, C.POINTER(FloorParams)]),
+    ("lsd_floor_destroy", _i, [_vp]),
+    ("lsd_floor_detect", _i, [_vp, _vp, _i, C.POINTER(FloorResult)]),
+    ("lsd_floor_detect_dev", _i, [_vp, _vp, _i, C.POINTER(FloorResult)]),
+    ("lsd_floor_get_cloud", _i, [_vp, _i, _vp, _i, _pi]),
+    ("lsd_floor_get_cloud_dev", _i, [_vp, _i, _pp, _pi]),
+    ("lsd_floor_get_normals", _i, [_vp, _vp, _vp, _i, _pi]),
+    ("lsd_floor_last_samples", _i, [_vp, _vp, _vp, _vp, _i, _pi]),
+    ("lsd_ransac_replay", _i, [_vp, _vp, _i, _i, _d, _i, _pi, _pi, _pi, _pi]),
     ("lsd_lio_init_cov", None, [_vp]),
     ("lsd_state_boxplus", None, [_vp, _vp]),
     ("lsd_state_boxminus", None, [_vp, _vp, _vp]),
@@ -891,6 +921,90 @@ def galign_merge_candidates(cand_idx, cand_dist, cand_shift, n_cand, dist_thres:
     check(lib.lsd_galign_merge_candidates(_ptr(idx), _ptr(dist), _ptr(sh), _ptr(nc), n_off, float(dist_thres), _ptr(oi), _ptr(od),
                                           _ptr(oy), cap, C.byref(n)))
     return oi[:n.value].copy(), od[:n.value].copy(), oy[:n.value].copy()
+
+
+def floor_params(preset: int = FLOOR_MAPPING, **kw) -> FloorParams:
+    p = FloorParams()
+    lib.lsd_floor_default_params(C.byref(p), int(preset))
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(f"lsd_floor_params_t has no field {k}")
+        setattr(p, k, v)
+    return p
+
+
+class FloorDetector:
+    """Floor detection on the device (FloorDetectionNodelet::detect and the two detect_ground copies): height clip,
+    k = 10 normal filter and RANSAC plane fit, one frame per detect().  preset: FLOOR_MAPPING (with the prefilter),
+    FLOOR_GROUND or FLOOR_RENDER; keyword arguments set lsd_floor_params_t fields."""
+
+    def __init__(self, preset: int = FLOOR_MAPPING, **kw):
+        self.h = None
+        self.params = floor_params(preset, **kw)
+        self.h = C.c_void_p()
+        check(lib.lsd_floor_create(C.byref(self.h), C.byref(self.params)))
+
+    def close(self):
+        if self.h:
+            lib.lsd_floor_destroy(self.h)
+        self.h = None
+
+    __del__ = close
+
+    def detect(self, pts) -> dict:
+        """One frame: [n,4] float32 (numpy: host input; torch CUDA tensor: device input).  Returns the result fields;
+        coeffs is float32[4] (upward normal when found)."""
+        r = FloorResult()
+        if isinstance(pts, np.ndarray):
+            a = _f32(pts)
+            check(lib.lsd_floor_detect(self.h, _ptr(a), a.shape[0], C.byref(r)))
+        else:
+            if str(pts.dtype) != "torch.float32" or pts.dim() != 2 or pts.shape[1] != 4 or not pts.is_contiguous():
+                raise ValueError("device points must be a contiguous float32 [n,4] tensor")
+            check(lib.lsd_floor_detect_dev(self.h, pts.data_ptr(), pts.shape[0], C.byref(r)))
+        out = {k: getattr(r, k) for k, _ in r._fields_}
+        out["coeffs"] = np.array(r.coeffs, np.float32)
+        out["found"] = bool(r.found)
+        return out
+
+    def cloud(self, stage: str) -> np.ndarray:
+        """The cloud of a stage of the last detect: 'prefiltered', 'clipped', 'candidates' or 'inliers'."""
+        s = FLOOR_STAGES[stage]
+        n = C.c_int()
+        check(lib.lsd_floor_get_cloud(self.h, s, None, 0, C.byref(n)))
+        out = np.zeros((max(n.value, 1), 4), np.float32)
+        check(lib.lsd_floor_get_cloud(self.h, s, _ptr(out), n.value, C.byref(n)))
+        return out[:n.value]
+
+    def normals(self):
+        """(normal4 [m,4] = nx, ny, nz, curvature; cov6 [m,6] = xx, xy, xz, yy, yz, zz) per clipped point of the last detect."""
+        n = C.c_int()
+        check(lib.lsd_floor_get_normals(self.h, None, None, 0, C.byref(n)))
+        nr, cv = np.zeros((max(n.value, 1), 4), np.float32), np.zeros((max(n.value, 1), 6), np.float32)
+        check(lib.lsd_floor_get_normals(self.h, _ptr(nr), _ptr(cv), n.value, C.byref(n)))
+        return nr[:n.value], cv[:n.value]
+
+    def samples(self):
+        """The hypotheses RANSAC drew in the last detect, in draw order: (idx [m,3], flags [m], counts [m])."""
+        n = C.c_int()
+        check(lib.lsd_floor_last_samples(self.h, None, None, None, 0, C.byref(n)))
+        m = max(n.value, 1)
+        idx, fl, cn = np.zeros((m, 3), np.int32), np.zeros(m, np.int32), np.zeros(m, np.int32)
+        check(lib.lsd_floor_last_samples(self.h, _ptr(idx), _ptr(fl), _ptr(cn), n.value, C.byref(n)))
+        return idx[:n.value], fl[:n.value], cn[:n.value]
+
+
+def ransac_replay(counts, flags, n_points: int, probability: float = 0.99, max_iterations: int = 10000) -> dict:
+    """RandomSampleConsensus::computeModel's stop rule on hypotheses in draw order (pure host).  consumed = -1: the loop
+    had not ended after the given hypotheses."""
+    cn = np.ascontiguousarray(counts, np.int32).ravel()
+    fl = np.ascontiguousarray(flags, np.int32).ravel()
+    if cn.size != fl.size:
+        raise ValueError("counts and flags differ in length")
+    c, b, it, sk = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    check(lib.lsd_ransac_replay(_ptr(cn), _ptr(fl), cn.size, int(n_points), float(probability), int(max_iterations), C.byref(c),
+                                C.byref(b), C.byref(it), C.byref(sk)))
+    return dict(consumed=c.value, best=b.value, iterations=it.value, skipped=sk.value)
 
 
 def eskf_update_table(state, P, HTH, HTh, n_eff, R=0.001, max_iterations=4, eps=0.001, literal=False, converge_log=None):

@@ -109,10 +109,17 @@ lsd_status_t lsd_knn_set_shape(lsd_map_t* m, int shape);
  * (lsd_map_insert*) calls; the LIO front-end keeps its own travel_distance (laserMapping.cpp:1289-1291) and needs no
  * call.  Evictions are applied inside the insert calls; lsd_map_evict waits for them and returns how many voxels were
  * evicted so far.  Not on tile-sharded maps, not together with the brick layout; with it on, map_incremental is
- * synchronous (lsd_lio_params::async_map_insert is ignored).  One corner is approximated: a voxel evicted and re-created
- * inside ONE map_incremental batch keeps the batch's points by id, not by list position. */
+ * synchronous (lsd_lio_params::async_map_insert is ignored).  A voxel evicted and re-created inside one batch keeps
+ * exactly the points iVox keeps: those the batch added after the voxel's last eviction, whatever their ids. */
 lsd_status_t lsd_map_enable_lru(lsd_map_t* m, uint64_t capacity, double max_distance);
 lsd_status_t lsd_map_set_travel_distance(lsd_map_t* m, double distance);
+/* Test tap: every point the table holds, voxel by voxel (table order), each voxel's points in storage order (its level-0
+ * line, then the overflow lines).  Per point: its voxel coordinates (decoded from the key), x, y, z, id, and whether it
+ * is a box-delete tombstone (lsd_map_delete_boxes: coordinates set to the quiet NaN 0x7fc00000).  *n_points = the number
+ * of stored points, tombstones included; at most `cap` are written (cap = 0 with null arrays asks for the count).
+ * Copies the whole table to the host (128 bytes per line): a read-back for tests, not for the per-scan path. */
+lsd_status_t lsd_map_dump(lsd_map_t* m, int32_t* voxel3 /*[n,3]*/, float* xyz3 /*[n,3]*/, int32_t* ids /*[n]*/,
+                          uint8_t* tombstone /*[n]*/, uint64_t cap, uint64_t* n_points);
 lsd_status_t lsd_map_evict(lsd_map_t* m, uint64_t* n_evicted_total);
 /* *saturated = 1 when the map refused points since the previous call (probe chain full, > 127 overflow lines in a
  * voxel, coordinates beyond +-2^18 voxels): a map that silently stopped growing degrades odometry, so poll this (the
@@ -279,6 +286,11 @@ lsd_status_t lsd_lio_get_matches(lsd_lio_t* l, int32_t* near_idx /*[n,5]*/, floa
 lsd_status_t lsd_lio_update(lsd_lio_t* l, double* state26_inout, double* P529_inout, lsd_lio_info_t* info);
 /* map_incremental at `state` using the neighbour lists of the last search. */
 lsd_status_t lsd_lio_map_incremental(lsd_lio_t* l, const double* state26, int* n_added);
+/* Test tap after a map_incremental: the decision per downsampled point (0 = not added, 1 = PointToAdd, 2 =
+ * PointNoNeedDownsample; laserMapping.cpp:523-576) and the travel distance the LIO front-end handed the map's LRU.
+ * With lsd_lio_get_matches' `world` this is enough to restate the scan's two AddPoints calls (laserMapping.cpp:571-572).
+ * Writes at most `cap` flags; *n = the number of downsampled points. */
+lsd_status_t lsd_lio_get_map_flags(lsd_lio_t* l, uint8_t* flags, int cap, int* n, double* travel_distance);
 /* The whole per-scan pass: load (+downsample) -> [seed map | update -> map_incremental]. */
 lsd_status_t lsd_lio_scan(lsd_lio_t* l, const float* scan_host, int n, double* state26_inout, double* P529_inout,
                           lsd_lio_info_t* info);

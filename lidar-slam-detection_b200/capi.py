@@ -142,6 +142,7 @@ SIGNATURES = [
     ("lsd_knn_set_shape", _i, [_vp, _i]),
     ("lsd_map_enable_lru", _i, [_vp, C.c_uint64, _d]),
     ("lsd_map_set_travel_distance", _i, [_vp, _d]),
+    ("lsd_map_dump", _i, [_vp, _vp, _vp, _vp, _vp, C.c_uint64, _pu64]),
     ("lsd_map_evict", _i, [_vp, _vp]),
     ("lsd_map_saturated", _i, [_vp, _pi, _vp]),
     ("lsd_map_enable_bricks", _i, [_vp, _i]),
@@ -179,6 +180,7 @@ SIGNATURES = [
     ("lsd_lio_get_matches", _i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     ("lsd_lio_update", _i, [_vp, _vp, _vp, C.POINTER(LioInfo)]),
     ("lsd_lio_map_incremental", _i, [_vp, _vp, _pi]),
+    ("lsd_lio_get_map_flags", _i, [_vp, _vp, _i, _pi, C.POINTER(_d)]),
     ("lsd_lio_scan", _i, [_vp, _vp, _i, _vp, _vp, C.POINTER(LioInfo)]),
     ("lsd_lio_scan_dev", _i, [_vp, _vp, _i, _vp, _vp, C.POINTER(LioInfo)]),
     ("lsd_lio_prefetch", _i, [_vp, _vp, _i]),
@@ -402,6 +404,20 @@ class HashVoxelMap:
 
     def set_travel_distance(self, d: float):
         check(lib.lsd_map_set_travel_distance(self.h, float(d)))
+
+    def dump(self):
+        """Every stored point (include/lsdreg.h::lsd_map_dump) -> dict of voxel [n,3] int32, xyz [n,3] float32, id [n]
+        int32, tombstone [n] bool; voxel by voxel, each voxel's points in storage order.  Copies the whole table."""
+        n = C.c_uint64()
+        check(lib.lsd_map_dump(self.h, None, None, None, None, 0, C.byref(n)))
+        m = max(n.value, 1)
+        vox = np.empty((m, 3), np.int32)
+        xyz = np.empty((m, 3), np.float32)
+        ids = np.empty(m, np.int32)
+        tomb = np.empty(m, np.uint8)
+        check(lib.lsd_map_dump(self.h, _ptr(vox), _ptr(xyz), _ptr(ids), _ptr(tomb), n.value, C.byref(n)))
+        k = n.value
+        return dict(voxel=vox[:k], xyz=xyz[:k], id=ids[:k], tombstone=tomb[:k].astype(bool))
 
     def evict(self) -> int:
         n = C.c_uint64()
@@ -1452,6 +1468,15 @@ class LioFrontend:
         world = np.empty((n, 4), np.float32)
         check(lib.lsd_lio_get_matches(self.h, _ptr(idx), _ptr(xyz), _ptr(cnt), _ptr(sel), _ptr(plane), _ptr(world)))
         return dict(idx=idx, xyz=xyz, cnt=cnt, selected=sel, plane=plane, world=world)
+
+    def get_map_flags(self):
+        """-> (flags [n] uint8, travel_distance): the last map_incremental's decision per downsampled point (0 = not added,
+        1 = PointToAdd, 2 = PointNoNeedDownsample) and the travel distance handed to the map's LRU."""
+        n, d = C.c_int(), C.c_double()
+        check(lib.lsd_lio_get_map_flags(self.h, None, 0, C.byref(n), C.byref(d)))
+        flags = np.empty(max(n.value, 1), np.uint8)
+        check(lib.lsd_lio_get_map_flags(self.h, _ptr(flags), n.value, C.byref(n), C.byref(d)))
+        return flags[:n.value], d.value
 
     def update(self, state: np.ndarray, P: np.ndarray):
         state = np.array(state, np.float64)

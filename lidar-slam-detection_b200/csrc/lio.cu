@@ -1234,9 +1234,11 @@ lsd_status_t lio_map_incremental(lsd_lio* l, const double* x, int use_near, int*
       LSD_CUDA(cudaMemcpyAsync(f.data(), l->d_flags, (size_t)n, cudaMemcpyDeviceToHost, st));
     }
     LSD_CUDA(cudaStreamSynchronize(st));
+    // the ids the kernel stored (two's-complement wrap past 2^31 - 1, as the device's int arithmetic gives)
     std::vector<float4> pts; std::vector<int> ids;
     for (int pass = 1; pass <= 2; pass++)
-      for (int i = 0; i < n; i++) if (f[i] == pass) { pts.push_back(w[i]); ids.push_back(l->next_id + i + (pass == 2 ? id_t2 : 0)); }
+      for (int i = 0; i < n; i++)
+        if (f[i] == pass) { pts.push_back(w[i]); ids.push_back((int)((unsigned)l->next_id + (unsigned)i + (pass == 2 ? (unsigned)id_t2 : 0u))); }
     l->map->lru->distance = l->travel;
     lsd_status_t e = map_lru_touch(l->map, pts.data(), ids.data(), (int)pts.size(), 0, st);
     if (e) return e;
@@ -1825,6 +1827,17 @@ lsd_status_t lsd_lio_load_scan(lsd_lio_t* l, const float* scan_host, int n, int 
   lsd_lio::Stage* sg = free_stage(l);
   LSD_CUDA(cudaMemcpyAsync(sg->buf, scan_host, (size_t)n * 16, cudaMemcpyHostToDevice, l->stream));
   return lsd_lio_load_scan_dev(l, reinterpret_cast<const float*>(sg->buf), n, downsample, n_down);
+}
+
+lsd_status_t lsd_lio_get_map_flags(lsd_lio_t* l, uint8_t* flags, int cap, int* n, double* travel_distance) {
+  if (!l || l->n_down < 0 || (cap > 0 && !flags)) return LSD_ERR_INVALID;
+  LSD_CUDA(cudaSetDevice(l->device));
+  const int c = std::min(cap, l->n_down);
+  if (c > 0) LSD_CUDA(cudaMemcpyAsync(flags, l->d_flags, (size_t)c, cudaMemcpyDeviceToHost, l->stream));
+  LSD_CUDA(cudaStreamSynchronize(l->stream));
+  if (n) *n = l->n_down;
+  if (travel_distance) *travel_distance = l->travel;
+  return LSD_OK;
 }
 
 lsd_status_t lsd_lio_get_down(lsd_lio_t* l, float* out_host, int cap, int* n_down) {

@@ -4,8 +4,8 @@
 //   AddPoints :231-256  -> map_insert_kernel      (open addressing, 64-bit atomicCAS claim,
 //                                                  atomicAdd slot claim, float4 stores)
 //   GetClosestPoint :139-171 -> knn_query_kernel   (knn.cuh)
-// The LRU list of the reference (ivox3d.h:246-255) is not reproduced: the table is sized for the
-// whole map in HBM (80 GB on an H100) instead of evicting at 100 000 voxels.
+// The table is sized for the whole map in HBM (80 GB on an H100); the reference's capacity / LRU eviction
+// (ivox3d.h:246-255) is available on request (lsd_map_enable_lru: map_lru_touch + map_evict_kernel below).
 #include <stdarg.h>
 #include <stdlib.h>
 
@@ -359,22 +359,30 @@ static lsd_status_t map_scratch(lsd_map* m, size_t bytes) {
 
 // ------------------------------------------------------------------ LRU eviction (IVox::AddPoints, ivox3d.h:246-255)
 // One thread per evicted voxel: its level-0 line and every overflow line are retired (key = kTombKey: the probe chains that
-// run through them stay intact, no query can match them), the counters follow.  keep_from != INT_MIN is the rare case of
-// a voxel evicted and re-created inside one batch: points with id >= keep_from belong to the new voxel and are
-// re-inserted (they claim a fresh line).
-struct MapEvict { unsigned long long key; int keep_from; int pad; };
-__global__ void __launch_bounds__(128) map_evict_kernel(MapView mv, const MapEvict* __restrict__ ev, int n_ev) {
+// run through them stay intact, no query can match them), the counters follow (`points` loses the live points only: a
+// box delete already took its tombstones off).
+// A voxel evicted and re-created inside one batch keeps exactly what iVox keeps: the points the batch added to it after
+// its last eviction.  The host lists them, keep[k0, k1) sorted by their (x, y, z, id) bit patterns; the kernel looks every
+// stored point up in that list, retires the lines and re-inserts the points it found (they claim fresh lines).  A listed
+// point the map had refused (voxel or table full) is not found, stays refused and is counted in `dropped` once.
+struct MapEvict { unsigned long long key; int k0, k1; };
+__host__ __device__ __forceinline__ bool keep_less(const uint4& a, const uint4& b) {
+  return a.x != b.x ? a.x < b.x : a.y != b.y ? a.y < b.y : a.z != b.z ? a.z < b.z : a.w < b.w;
+}
+__device__ __forceinline__ bool is_tombstone(const float4& p) {   // map_delete_boxes_kernel's pattern
+  return __float_as_uint(p.x) == 0x7fc00000u && __float_as_uint(p.y) == 0x7fc00000u && __float_as_uint(p.z) == 0x7fc00000u;
+}
+__global__ void __launch_bounds__(128) map_evict_kernel(MapView mv, const MapEvict* __restrict__ ev, int n_ev,
+                                                        const uint4* __restrict__ keep, unsigned char* __restrict__ found) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n_ev) return;
   const unsigned long long key0 = ev[e].key;
-  const int keep_from = ev[e].keep_from;
+  const int k0 = ev[e].k0, k1 = ev[e].k1;
   uint4 h;
   const CellLine* base = tag_find(mv, key0, &h);
   if (!base) return;
   const unsigned total = h.z;
   const int levels = total > (unsigned)kPtsPerLine ? min((int)((total - 1) / kPtsPerLine), kMaxLevel) : 0;
-  float4 keep[8];
-  int nk = 0;
   unsigned long long stored = 0;
   for (int L = 0; L <= levels; L++) {
     CellLine* ln = const_cast<CellLine*>(base);
@@ -382,8 +390,14 @@ __global__ void __launch_bounds__(128) map_evict_kernel(MapView mv, const MapEvi
     const int n = (int)min(total - (unsigned)(L * kPtsPerLine), (unsigned)kPtsPerLine);
     for (int j = 0; j < n; j++) {
       const float4 p = ln->pts[j];
+      if (is_tombstone(p)) continue;
       stored++;
-      if (keep_from != (int)0x80000000 && __float_as_int(p.w) >= keep_from && nk < 8) keep[nk++] = p;
+      if (k0 == k1) continue;
+      const uint4 u = make_uint4(__float_as_uint(p.x), __float_as_uint(p.y), __float_as_uint(p.z), __float_as_uint(p.w));
+      int lo = k0, hi = k1;                                  // first listed entry not below u
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (keep_less(keep[mid], u)) lo = mid + 1; else hi = mid; }
+      for (; lo < k1 && !keep_less(u, keep[lo]); lo++)       // equal entries (exact duplicates): the first one not yet found
+        if (!found[lo]) { found[lo] = 1; break; }
     }
     ln->count = 0u;
     ln->key = kTombKey;
@@ -391,7 +405,8 @@ __global__ void __launch_bounds__(128) map_evict_kernel(MapView mv, const MapEvi
   atomicAdd(&mv.counters[0], ~0ull);                       // cells - 1
   atomicAdd(&mv.counters[1], 0ull - stored);
   __threadfence();
-  for (int j = 0; j < nk; j++) map_insert_point(mv, keep[j].x, keep[j].y, keep[j].z, __float_as_int(keep[j].w));
+  for (int q = k0; q < k1; q++)
+    if (found[q]) map_insert_point(mv, __uint_as_float(keep[q].x), __uint_as_float(keep[q].y), __uint_as_float(keep[q].z), (int)keep[q].w);
 }
 
 // Fresh table without the retired lines: every live line is copied to its place in the new table (whole 128-byte lines:
@@ -411,8 +426,17 @@ __global__ void __launch_bounds__(256) map_rehash_kernel(MapView src, unsigned l
   for (int j = 0; j < kPtsPerLine; j++) out->pts[j] = ln->pts[j];
 }
 
+// pos2grid as the device evaluates it.  The device's float -> int conversion saturates and turns NaN into 0, so a point with
+// a NaN coordinate lands in voxel 0 along that axis (x86's conversion gives INT_MIN for both).  The LRU mirror must file
+// every point where map_insert_point filed it.
+static __host__ int device_f2i(float v) {
+  if (v != v) return 0;
+  if (v >= 2147483648.0f) return 0x7fffffff;
+  if (v < -2147483648.0f) return (int)0x80000000;
+  return (int)v;
+}
 static __host__ int3 pos2grid_host(float x, float y, float z, float inv_res) {
-  return make_int3((int)roundf(x * inv_res), (int)roundf(y * inv_res), (int)roundf(z * inv_res));
+  return make_int3(device_f2i(roundf(x * inv_res)), device_f2i(roundf(y * inv_res)), device_f2i(roundf(z * inv_res)));
 }
 
 static lsd_status_t map_rehash(lsd_map* m, cudaStream_t st) {
@@ -437,6 +461,7 @@ lsd_status_t map_lru_touch(lsd_map* m, const float4* pts, const int* ids, int n,
   LruMirror* L = m->lru;
   if (!L || n <= 0) return LSD_OK;
   std::vector<MapEvict> ev;
+  std::vector<std::vector<int>> survivors;                   // per entry of ev: batch positions added after its last eviction
   std::unordered_map<unsigned long long, size_t> in_batch;   // key -> its entry in ev (evicted during this batch)
   const float inv = m->view.inv_res;
   for (int i = 0; i < n; i++) {
@@ -448,28 +473,49 @@ lsd_status_t map_lru_touch(lsd_map* m, const float4* pts, const int* ids, int n,
     if (it == L->idx.end()) {
       L->cache.push_front({key, L->distance});
       L->idx[key] = L->cache.begin();
-      auto b = in_batch.find(key);
-      if (b != in_batch.end()) ev[b->second].keep_from = ids ? ids[i] : id0 + i;   // evicted earlier in this batch, re-created now
     } else {
       L->cache.splice(L->cache.begin(), L->cache, it->second);
     }
+    auto b = in_batch.find(key);
+    if (b != in_batch.end()) survivors[b->second].push_back(i);   // evicted earlier in this batch and alive again
     if (L->idx.size() > L->capacity && (L->distance - L->cache.back().d0) > L->max_distance) {
       const unsigned long long k = L->cache.back().key;
       L->idx.erase(k);
       L->cache.pop_back();
-      auto b = in_batch.find(k);
-      if (b != in_batch.end()) ev[b->second].keep_from = (int)0x80000000;     // evicted again: nothing of it survives
-      else { in_batch[k] = ev.size(); ev.push_back({k, (int)0x80000000, 0}); }
+      auto e = in_batch.find(k);
+      if (e != in_batch.end()) survivors[e->second].clear();     // evicted again: nothing added so far survives
+      else { in_batch[k] = ev.size(); ev.push_back({k, 0, 0}); survivors.emplace_back(); }
       L->n_evicted++;
     }
   }
   if (ev.empty()) return LSD_OK;
-  lsd_status_t s = map_scratch(m, ev.size() * sizeof(MapEvict));
+  // the points to keep, as the device stores them: (x, y, z, id) bit patterns, sorted per voxel for the kernel's lookup
+  std::vector<uint4> keep;
+  for (size_t e = 0; e < ev.size(); e++) {
+    ev[e].k0 = (int)keep.size();
+    for (int i : survivors[e]) {
+      uint4 u;
+      memcpy(&u, &pts[i], 12);
+      u.w = ids ? (unsigned)ids[i] : (unsigned)id0 + (unsigned)i;
+      keep.push_back(u);
+    }
+    ev[e].k1 = (int)keep.size();
+    std::sort(keep.begin() + ev[e].k0, keep.end(), keep_less);
+  }
+  const size_t o_keep = (ev.size() * sizeof(MapEvict) + 15) & ~(size_t)15, o_found = o_keep + keep.size() * sizeof(uint4);
+  lsd_status_t s = map_scratch(m, o_found + keep.size() + 1);
   if (s) return s;
-  LSD_CUDA(cudaMemcpyAsync(m->scratch, ev.data(), ev.size() * sizeof(MapEvict), cudaMemcpyHostToDevice, st));
-  map_evict_kernel<<<(unsigned)((ev.size() + 127) / 128), 128, 0, st>>>(m->view, static_cast<const MapEvict*>(m->scratch), (int)ev.size());
+  char* sc = static_cast<char*>(m->scratch);
+  LSD_CUDA(cudaMemcpyAsync(sc, ev.data(), ev.size() * sizeof(MapEvict), cudaMemcpyHostToDevice, st));
+  if (!keep.empty()) {
+    LSD_CUDA(cudaMemcpyAsync(sc + o_keep, keep.data(), keep.size() * sizeof(uint4), cudaMemcpyHostToDevice, st));
+    LSD_CUDA(cudaMemsetAsync(sc + o_found, 0, keep.size(), st));
+  }
+  map_evict_kernel<<<(unsigned)((ev.size() + 127) / 128), 128, 0, st>>>(m->view, reinterpret_cast<const MapEvict*>(sc), (int)ev.size(),
+                                                                        reinterpret_cast<const uint4*>(sc + o_keep),
+                                                                        reinterpret_cast<unsigned char*>(sc + o_found));
   LSD_CUDA(cudaGetLastError());
-  LSD_CUDA(cudaStreamSynchronize(st));                        // `ev` lives on this stack frame
+  LSD_CUDA(cudaStreamSynchronize(st));                        // `ev` and `keep` live on this stack frame
   m->launches++;
   L->tombstones += ev.size();
   // retired lines keep their slots: rebuild the table before they crowd the probe chains
@@ -733,6 +779,48 @@ lsd_status_t lsd_map_stats(lsd_map_t* m, uint64_t* n_cells, uint64_t* n_points, 
   if (n_cells) *n_cells = h[0];
   if (n_points) *n_points = h[1];
   if (n_dropped) *n_dropped = h[2];
+  return LSD_OK;
+}
+
+lsd_status_t lsd_map_dump(lsd_map_t* m, int32_t* voxel3, float* xyz3, int32_t* ids, uint8_t* tombstone, uint64_t cap,
+                          uint64_t* n_points) {
+  if (!m || !n_points || (cap > 0 && (!voxel3 || !xyz3 || !ids || !tombstone))) return LSD_ERR_INVALID;
+  LSD_CUDA(cudaSetDevice(m->device));
+  std::vector<CellLine> t((size_t)m->n_lines);
+  LSD_CUDA(cudaMemcpyAsync(t.data(), m->view.lines, (size_t)m->n_lines * sizeof(CellLine), cudaMemcpyDeviceToHost, m->stream));
+  LSD_CUDA(cudaStreamSynchronize(m->stream));
+  std::unordered_map<unsigned long long, size_t> over;   // overflow line key -> slot
+  for (size_t s = 0; s < t.size(); s++)
+    if (t[s].key != 0ull && t[s].key != kTombKey && (t[s].key >> 57) != 0ull) over[t[s].key] = s;
+  uint64_t k = 0;
+  for (size_t s = 0; s < t.size(); s++) {
+    const unsigned long long key = t[s].key;
+    if (key == 0ull || key == kTombKey || (key >> 57) != 0ull) continue;
+    const int v[3] = {(int)((key >> 38) & 0x7ffffull) - kCoordBias, (int)((key >> 19) & 0x7ffffull) - kCoordBias,
+                      (int)(key & 0x7ffffull) - kCoordBias};
+    const unsigned total = t[s].count;
+    const int levels = total > (unsigned)kPtsPerLine ? std::min((int)((total - 1) / kPtsPerLine), kMaxLevel) : 0;
+    for (int L = 0; L <= levels; L++) {
+      const CellLine* ln = &t[s];
+      if (L > 0) {
+        auto it = over.find(key | ((unsigned long long)L << 57));
+        if (it == over.end()) continue;
+        ln = &t[it->second];
+      }
+      const int n = (int)std::min(total - (unsigned)(L * kPtsPerLine), (unsigned)kPtsPerLine);
+      for (int j = 0; j < n; j++, k++) {
+        if (k >= cap) continue;
+        const float4 p = ln->pts[j];
+        unsigned b[3];
+        memcpy(b, &p, 12);
+        for (int d = 0; d < 3; d++) voxel3[3 * k + d] = v[d];
+        xyz3[3 * k] = p.x; xyz3[3 * k + 1] = p.y; xyz3[3 * k + 2] = p.z;
+        memcpy(&ids[k], &p.w, 4);
+        tombstone[k] = b[0] == 0x7fc00000u && b[1] == 0x7fc00000u && b[2] == 0x7fc00000u;
+      }
+    }
+  }
+  *n_points = k;
   return LSD_OK;
 }
 

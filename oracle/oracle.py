@@ -82,11 +82,17 @@ def _load_ref():
         return None
     L = C.CDLL(_REF)
     L.ref_ivox_create.restype = C.c_void_p
-    L.ref_ivox_create.argtypes = [C.c_float, C.c_int, C.c_size_t]
+    L.ref_ivox_create.argtypes = [C.c_float, C.c_int, C.c_size_t, C.c_double]
     L.ref_ivox_destroy.argtypes = [C.c_void_p]
     L.ref_ivox_add.argtypes = [C.c_void_p, _f, C.c_int, C.c_int, C.c_double]
     L.ref_ivox_num_cells.restype = C.c_size_t
     L.ref_ivox_num_cells.argtypes = [C.c_void_p]
+    if hasattr(L, "ref_ivox_dump"):        # a library built from an older ref_lio.cpp lacks them (see HAVE_REF_IVOX_DUMP)
+        L.ref_ivox_add_ids.argtypes = [C.c_void_p, _f, _i, C.c_int, C.c_double]
+        L.ref_ivox_num_points.restype = C.c_size_t
+        L.ref_ivox_num_points.argtypes = [C.c_void_p]
+        L.ref_ivox_dump.restype = C.c_size_t
+        L.ref_ivox_dump.argtypes = [C.c_void_p, C.c_float, _i, _f, _i, C.c_size_t]
     if hasattr(L, "ref_ivox_set_nearby"):
         L.ref_ivox_set_nearby.argtypes = [C.c_void_p, C.c_int]
     L.ref_ivox_knn.argtypes = [C.c_void_p, _f, C.c_int, C.c_int, C.c_double, _i, _f, _i, C.c_int]
@@ -213,6 +219,8 @@ def _load_ref_ikfom():
 port = _load_port()
 ref = _load_ref()
 HAVE_REF = ref is not None
+# the compiled iVox with a settable max_distance, explicit ids and the content dump (ref_lio.cpp's newer entry points)
+HAVE_REF_IVOX_DUMP = HAVE_REF and hasattr(ref, "ref_ivox_dump")
 ref_reg = _load_ref_reg()
 HAVE_REF_REG = ref_reg is not None
 ref_ikfom = _load_ref_ikfom()
@@ -296,9 +304,12 @@ def esti_plane(pts5: np.ndarray, thr: float = 0.1):
 class RefIvox:
     """The reference's own faster_lio::IVox, compiled unmodified (oracle/_ref)."""
 
-    def __init__(self, res: float = 0.5, nearby: int = 18, capacity: int = 1 << 30):
+    def __init__(self, res: float = 0.5, nearby: int = 18, capacity: int = 1 << 30, max_distance: float = 100.0):
         assert HAVE_REF, "oracle/_ref/libref_lio.so not built"
-        self.h = ref.ref_ivox_create(res, nearby, capacity)
+        # an older library hard-wires max_distance = 100 (the extra argument is then ignored)
+        assert HAVE_REF_IVOX_DUMP or max_distance == 100.0, "oracle/_ref/libref_lio.so predates ref_ivox_create's max_distance"
+        self.res = res
+        self.h = ref.ref_ivox_create(res, nearby, capacity, float(max_distance))
 
     def __del__(self):
         if getattr(self, "h", None):
@@ -310,12 +321,34 @@ class RefIvox:
         xyz = _c32(xyz[:, :3])
         ref.ref_ivox_add(self.h, xyz, xyz.shape[0], id0, float(distance))
 
+    def add_ids(self, xyz: np.ndarray, ids: np.ndarray, distance: float = 0.0):
+        """AddPoints with an explicit id per point."""
+        xyz = _c32(xyz[:, :3])
+        ids = np.ascontiguousarray(ids, np.int32)
+        assert ids.shape == (xyz.shape[0],)
+        ref.ref_ivox_add_ids(self.h, xyz, ids, xyz.shape[0], float(distance))
+
     def set_nearby(self, nearby: int):
         ref.ref_ivox_set_nearby(self.h, nearby)
 
     @property
     def num_cells(self):
         return ref.ref_ivox_num_cells(self.h)
+
+    @property
+    def num_points(self):
+        return ref.ref_ivox_num_points(self.h)
+
+    def dump(self):
+        """-> keys [n,3] int32, xyz [n,3] float32, ids [n] int32: every stored point (IVox::GetAllPoints), each voxel's
+        points in insertion order; keys are computed by Pos2Grid's expression in C++ (Eigen rounds half away from zero)."""
+        n = ref.ref_ivox_num_points(self.h)
+        keys = np.empty((max(n, 1), 3), np.int32)
+        xyz = np.empty((max(n, 1), 3), np.float32)
+        ids = np.empty(max(n, 1), np.int32)
+        m = ref.ref_ivox_dump(self.h, self.res, keys, xyz, ids, n)
+        assert m == n
+        return keys[:n], xyz[:n], ids[:n]
 
     def knn(self, q: np.ndarray, k: int = 5, max_sq: float = 5.0, nthreads: int = 8):
         """-> ids [nq,k], xyz [nq,k,3], cnt [nq] in the REFERENCE's order (nearest first)."""

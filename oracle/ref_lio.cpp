@@ -33,11 +33,11 @@ static inline int id_of(const PointType& p) { return int(p.normal_x) | (int(p.no
 extern "C" {
 
 // ---------------------------------------------------------------- iVox
-void* ref_ivox_create(float res, int nearby, size_t capacity) {
+void* ref_ivox_create(float res, int nearby, size_t capacity, double max_distance) {
   IVoxType::Options o;
   o.resolution_ = res;
   o.capacity_ = capacity;
-  o.max_distance_ = 100.0;
+  o.max_distance_ = max_distance;
   switch (nearby) {
     case 0: o.nearby_type_ = IVoxType::NearbyType::CENTER; break;
     case 6: o.nearby_type_ = IVoxType::NearbyType::NEARBY6; break;
@@ -55,7 +55,35 @@ void ref_ivox_add(void* h, const float* xyz, int n, int id0, double distance) {
   for (int i = 0; i < n; i++) pv.push_back(mk(xyz + 3 * i, id0 + i));
   static_cast<IVoxType*>(h)->AddPoints(pv, distance);
 }
+// AddPoints with explicit ids (the LIO front-end's two calls per scan carry ids that are not one run id0 + i)
+void ref_ivox_add_ids(void* h, const float* xyz, const int* ids, int n, double distance) {
+  PointVector pv;
+  pv.reserve(n);
+  for (int i = 0; i < n; i++) pv.push_back(mk(xyz + 3 * i, ids[i]));
+  static_cast<IVoxType*>(h)->AddPoints(pv, distance);
+}
 size_t ref_ivox_num_cells(void* h) { return static_cast<IVoxType*>(h)->NumValidGrids(); }
+size_t ref_ivox_num_points(void* h) {
+  IVoxType::PointVector all;
+  static_cast<IVoxType*>(h)->GetAllPoints(all);
+  return all.size();
+}
+// Every stored point (IVox::GetAllPoints: voxel by voxel, each voxel's points in insertion order) with its voxel key.
+// The key is Pos2Grid's own expression (ivox3d.h:259), evaluated here so that Eigen's rounding (half away from zero) and
+// its float -> int conversion are the reference's; `res` is the resolution the map was created with, and the inverse is
+// formed as the constructor forms options_.inv_resolution_ (ivox3d.h:58).  Returns the number of points; writes at most cap.
+size_t ref_ivox_dump(void* h, float res, int* key3, float* xyz, int* ids, size_t cap) {
+  IVoxType::PointVector all;
+  static_cast<IVoxType*>(h)->GetAllPoints(all);
+  const float inv = 1.0 / res;
+  for (size_t i = 0; i < all.size() && i < cap; i++) {
+    const Eigen::Matrix<float, 3, 1> p(all[i].x, all[i].y, all[i].z);
+    const Eigen::Matrix<int, 3, 1> k = (p * inv).array().round().template cast<int>();
+    for (int d = 0; d < 3; d++) { key3[3 * i + d] = k(d); xyz[3 * i + d] = (&all[i].x)[d]; }
+    ids[i] = id_of(all[i]);
+  }
+  return all.size();
+}
 // IVox::SetNearByType (ivox3d.h:64-67): the pipeline starts on NEARBY74 and switches to NEARBY18 (laserMapping.cpp:1241-1243)
 void ref_ivox_set_nearby(void* h, int nearby) {
   IVoxType::NearbyType t = IVoxType::NearbyType::NEARBY74;

@@ -24,6 +24,7 @@ _CASES = {
     "fuzz_misc": ("simt/fuzz_misc.py", "FUZZ_MISC_OK"),
     "fuzz_reforder": ("simt/fuzz_reforder.py", "FUZZ_REFORDER_OK"),   # reference-order rows on crowded / clustered maps, every path of the search kernel
     "fuzz_nth": ("simt/fuzz_nth.py", "FUZZ_NTH_OK"),   # std::nth_element as the search kernel replays it vs the restatement (warp path, depth-limit bail-out, serial path)
+    "fuzz_map_contents": ("simt/fuzz_map_contents.py", "FUZZ_MAP_CONTENTS_OK"),   # the map's contents voxel by voxel: insert, box delete, LRU eviction
     "fuzz_pipeline": ("simt/fuzz_pipeline.py", "FUZZ_PIPELINE_OK"),   # random announce / register schedules: staging slots, deferred requests, buffer hand-over   # voxel grid, key-frame filters, ScanContext descriptor on degenerate inputs
 }
 

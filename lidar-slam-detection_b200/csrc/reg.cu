@@ -33,6 +33,10 @@ namespace lsd {
 
 // ------------------------------------------------------------------ NDT voxel table
 struct __align__(128) NdtBuildLine { unsigned long long key; unsigned count; unsigned pad; double sum[3]; double sxx[6]; };
+// The VGICP build table sums in 128-bit fixed point (2^-64 resolution: hi = integer part, lo = fraction).  Integer addition
+// is associative, so a voxel's sums do not depend on the order in which its points' atomics land: every build of the same
+// cloud gives the same table bits, and so do the single-pair matcher and the closure search, which build their own.
+struct __align__(32) VgBuildLine { unsigned long long key; unsigned count; unsigned pad; unsigned long long lo[9]; unsigned long long hi[9]; };
 struct __align__(64) NdtLine { unsigned long long key; int n; float mean[3]; float nrm[3]; float pad[7]; };
 static_assert(sizeof(NdtLine) == 64, "NdtLine must be two sectors");
 
@@ -45,7 +49,8 @@ __device__ __forceinline__ int3 ndt_coord(float x, float y, float z, float res) 
 
 // The build-table slot of voxel `key` (open addressing, linear probing), claimed if the voxel is new; -1 when kMaxProbe
 // probes find neither the key nor a free slot.  Both voxel maps (NDT, VGICP) are accumulated through here.
-__device__ __forceinline__ long long claim_slot(NdtBuildLine* __restrict__ tab, unsigned long long mask, unsigned long long key) {
+template <class Line>
+__device__ __forceinline__ long long claim_slot(Line* __restrict__ tab, unsigned long long mask, unsigned long long key) {
   unsigned long long s = hash_key(key) & mask;
   for (unsigned probe = 0; probe < kMaxProbe; probe++) {
     unsigned long long* kp = &tab[s].key;
@@ -488,8 +493,23 @@ __device__ __forceinline__ int3 vg_coord(double x, double y, double z, double re
   return make_int3((int)floor(x / res - 0.5), (int)floor(y / res - 0.5), (int)floor(z / res - 0.5));
 }
 
+// v (|v| < 2^63) to the fixed point of VgBuildLine, rounded down at 2^-64; the words are added with the carry out of the low one
+__device__ __forceinline__ void fixed_add(unsigned long long* lo, unsigned long long* hi, double v) {
+  const double fl = floor(v);
+  double f = v - fl;                                   // rounds up to 1.0 only for tiny negative v
+  unsigned long long h = (unsigned long long)(long long)fl;
+  if (f >= 1.0) { f = 0.0; h += 1ull; }
+  const unsigned long long l = (unsigned long long)(f * 18446744073709551616.0);   // [0, 1) * 2^64
+  const unsigned long long old = atomicAdd(lo, l);
+  atomicAdd(hi, h + (old + l < old ? 1ull : 0ull));
+}
+
+__device__ __forceinline__ double fixed_value(unsigned long long lo, unsigned long long hi) {
+  return (double)(long long)hi + (double)lo * 5.421010862427522e-20;   // lo * 2^-64
+}
+
 // GaussianVoxelMap::create_voxelmap: sum[] = sum of points, sxx[] = sum of covariances (xx xy xz yy yz zz)
-__global__ void __launch_bounds__(256) vgicp_accum_kernel(NdtBuildLine* __restrict__ tab, unsigned long long mask, double res,
+__global__ void __launch_bounds__(256) vgicp_accum_kernel(VgBuildLine* __restrict__ tab, unsigned long long mask, double res,
                                                           const float4* __restrict__ pts, const double* __restrict__ nrm, int n,
                                                           unsigned* __restrict__ fail) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -502,13 +522,13 @@ __global__ void __launch_bounds__(256) vgicp_accum_kernel(NdtBuildLine* __restri
   if (s < 0) { atomicAdd(fail, 1u); return; }
   const double nx = nrm[4 * (size_t)i], ny = nrm[4 * (size_t)i + 1], nz = nrm[4 * (size_t)i + 2];
   atomicAdd(&tab[s].count, 1u);
-  atomicAdd(&tab[s].sum[0], x); atomicAdd(&tab[s].sum[1], y); atomicAdd(&tab[s].sum[2], z);
-  atomicAdd(&tab[s].sxx[0], 1.0 - 0.999 * nx * nx); atomicAdd(&tab[s].sxx[1], -0.999 * nx * ny); atomicAdd(&tab[s].sxx[2], -0.999 * nx * nz);
-  atomicAdd(&tab[s].sxx[3], 1.0 - 0.999 * ny * ny); atomicAdd(&tab[s].sxx[4], -0.999 * ny * nz); atomicAdd(&tab[s].sxx[5], 1.0 - 0.999 * nz * nz);
+  const double v[9] = {x, y, z, 1.0 - 0.999 * nx * nx, -0.999 * nx * ny, -0.999 * nx * nz, 1.0 - 0.999 * ny * ny, -0.999 * ny * nz, 1.0 - 0.999 * nz * nz};
+#pragma unroll
+  for (int k = 0; k < 9; k++) fixed_add(&tab[s].lo[k], &tab[s].hi[k], v[k]);
 }
 
 // AdditiveGaussianVoxel::finalize
-__global__ void __launch_bounds__(256) vgicp_finalize_kernel(const NdtBuildLine* __restrict__ tab, VgLine* __restrict__ out,
+__global__ void __launch_bounds__(256) vgicp_finalize_kernel(const VgBuildLine* __restrict__ tab, VgLine* __restrict__ out,
                                                              unsigned long long n_lines, unsigned* __restrict__ n_vox) {
   const unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n_lines) return;
@@ -520,8 +540,8 @@ __global__ void __launch_bounds__(256) vgicp_finalize_kernel(const NdtBuildLine*
   if (o.key != 0ull) {
     const double n = (double)tab[s].count;
     o.n = (int)tab[s].count;
-    for (int k = 0; k < 3; k++) o.mean[k] = tab[s].sum[k] / n;
-    for (int k = 0; k < 6; k++) o.cov[k] = tab[s].sxx[k] / n;
+    for (int k = 0; k < 3; k++) o.mean[k] = fixed_value(tab[s].lo[k], tab[s].hi[k]) / n;
+    for (int k = 0; k < 6; k++) o.cov[k] = fixed_value(tab[s].lo[3 + k], tab[s].hi[3 + k]) / n;
     atomicAdd(n_vox, 1u);
   }
   out[s] = o;
@@ -1041,15 +1061,15 @@ static int auto_log2(size_t n_items, int lo, int hi) {
 // The target's voxel map v (NdtView or VgView, v.res already set) for n points: sized from n (or map_log2_lines), its
 // build table allocated and cleared, accum(build, mask, d_fail) and finalize(build, lines, d_vox) launched on the
 // handle's stream.  Fails with LSD_ERR_CAPACITY when a point found no slot or lies outside the key range.
-template <class View, class Accum, class Finalize>
+template <class Line, class View, class Accum, class Finalize>
 static lsd_status_t build_voxel_table(lsd_reg* r, int n, const char* method, View& v, unsigned long long& n_lines, Accum accum,
                                       Finalize finalize) {
   cudaStream_t st = r->stream;
   const int l2 = r->p.map_log2_lines > 0 ? r->p.map_log2_lines : auto_log2((size_t)n / 2 + 1024, 12, 27);
   const unsigned long long lines = 1ull << l2;
-  NdtBuildLine* build = nullptr;
-  LSD_CUDA(cudaMalloc((void**)&build, lines * sizeof(NdtBuildLine)));
-  LSD_CUDA(cudaMemsetAsync(build, 0, lines * sizeof(NdtBuildLine), st));
+  Line* build = nullptr;
+  LSD_CUDA(cudaMalloc((void**)&build, lines * sizeof(Line)));
+  LSD_CUDA(cudaMemsetAsync(build, 0, lines * sizeof(Line), st));
   if (n_lines != lines) {
     cudaFree(v.lines); v.lines = nullptr;
     LSD_CUDA(cudaMalloc((void**)&v.lines, lines * sizeof(*v.lines)));
@@ -1262,11 +1282,11 @@ static lsd_status_t gicp_covariances(lsd_reg* r, lsd_map** mp, const float4* d_p
 static lsd_status_t vgicp_voxel_table(lsd_reg* r, const float4* d_pts, const double* nrm, int n, VgView& vg, unsigned long long& vg_lines) {
   cudaStream_t st = r->stream;
   vg.res = r->p.resolution;
-  return build_voxel_table(r, n, "VGICP", vg, vg_lines,
-      [&](NdtBuildLine* build, unsigned long long mask, unsigned* d_fail) {
+  return build_voxel_table<VgBuildLine>(r, n, "VGICP", vg, vg_lines,
+      [&](VgBuildLine* build, unsigned long long mask, unsigned* d_fail) {
         vgicp_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, mask, vg.res, d_pts, nrm, n, d_fail);
       },
-      [&](const NdtBuildLine* build, unsigned long long lines, unsigned* d_vox) {
+      [&](const VgBuildLine* build, unsigned long long lines, unsigned* d_vox) {
         vgicp_finalize_kernel<<<(unsigned)((lines + 255) / 256), 256, 0, st>>>(build, vg.lines, lines, d_vox);
       });
 }
@@ -1288,7 +1308,7 @@ lsd_status_t lsd_reg_set_target_dev(lsd_reg_t* r, const float* pts_dev, int n) {
   r->tgt_map_built = false;
   if (r->p.kind == LSD_REG_NDT_P2D) {
     r->ndt.res = (float)r->p.resolution;
-    lsd_status_t s = build_voxel_table(r, n, "NDT", r->ndt, r->ndt_lines,
+    lsd_status_t s = build_voxel_table<NdtBuildLine>(r, n, "NDT", r->ndt, r->ndt_lines,
         [&](NdtBuildLine* build, unsigned long long mask, unsigned* d_fail) {
           ndt_accum_kernel<<<(n + 255) / 256, 256, 0, st>>>(build, mask, r->ndt.res, r->d_tgt, n, d_fail, r->sc.rank, r->sc.world, r->shard_tile);
         },

@@ -60,7 +60,7 @@ __global__ void __launch_bounds__(256) vgicp_cost_batch_kernel(const float4* __r
 // getFitnessScore(max_range) of every pair at its pose against its reference key frame's point map: per pair the shape,
 // grid and body of lsd_reg_fitness (fitness_range, reg.cu) and its fold, so the same sum and count.
 __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_pairs_kernel(const float4* __restrict__ pool, const GaCand* __restrict__ cands,
-                                                                          int n_cand, float search_sq, float max_range,
+                                                                          int n_cand, float search_sq, double max_range,
                                                                           double* __restrict__ partials, unsigned* __restrict__ done,
                                                                           double* __restrict__ result, double seq) {
   const int c = loop_cand_of_block(cands, n_cand);
@@ -204,7 +204,7 @@ static lsd_status_t ga_fitness(lsd_galign* h, const std::vector<GaPair>& pairs, 
   if (s) return s;
   const double max_range = h->p.fitness_score_max_range;
   fitness_pairs_kernel<<<blocks, kRegWarps * 32, 0, st>>>(h->d_pool, h->b.d_cand, n, fitness_search_sq(max_range, h->p.reg.map_resolution),
-                                                          (float)max_range, h->b.d_partials, h->b.d_done, h->b.d_res, seq);
+                                                          max_range, h->b.d_partials, h->b.d_done, h->b.d_res, seq);
   LSD_CUDA(cudaGetLastError());
   (*launches)++;
   s = h->b.wait(st, seq);

@@ -109,7 +109,7 @@ __global__ void __launch_bounds__(256) ndt_cost_batch_kernel(NdtView v, const fl
 // tgt != nullptr: points with no neighbour within search_sq get the exact one, for calc_fitness_score.
 __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_batch_kernel(MapView mv, const float4* __restrict__ pool,
                                                                           const LoopCand* __restrict__ cands, int n_cand, float search_sq,
-                                                                          float max_range, const float4* __restrict__ tgt, int n_tgt,
+                                                                          double max_range, const float4* __restrict__ tgt, int n_tgt,
                                                                           double* __restrict__ partials, unsigned* __restrict__ done,
                                                                           double* __restrict__ result, double seq) {
   const int c = loop_cand_of_block(cands, n_cand);
@@ -260,7 +260,7 @@ static lsd_status_t loop_fitness(lsd_loop* h, const std::vector<int>& slots, con
   s = h->b.upload(n, st, &seq);
   if (s) return s;
   const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
-  fitness_batch_kernel<<<blocks, kRegWarps * 32, 0, st>>>(r->tgt_map->view, h->d_pool, h->b.d_cand, n, search_sq, (float)max_range,
+  fitness_batch_kernel<<<blocks, kRegWarps * 32, 0, st>>>(r->tgt_map->view, h->d_pool, h->b.d_cand, n, search_sq, max_range,
                                                          exact ? r->d_tgt : nullptr, r->n_tgt, h->b.d_partials, h->b.d_done, h->b.d_res, seq);
   LSD_CUDA(cudaGetLastError());
   (*launches)++;

@@ -393,11 +393,13 @@ __device__ __forceinline__ void gicp_store_maha(const double* __restrict__ src_n
 }
 
 // update_correspondences (fast_gicp_impl.hpp:119-157): 1-NN of the transformed source point, Mahalanobis
-// matrix.  One warp per source point.
+// matrix.  One warp per source point.  The reference keeps the neighbour when its FLOAT squared distance is below the DOUBLE
+// max_corr_dist^2 (fast_gicp_impl.hpp:141): gate with max_corr_sq in double; search_sq (corr_search_sq) is the inclusive
+// float bound of the grid search that holds every float below it.
 __global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv, const float4* __restrict__ src,
                                                                       const double* __restrict__ src_nrm, int n,
                                                                       const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
-                                                                      float max_corr_sq, int* __restrict__ corr,
+                                                                      float search_sq, double max_corr_sq, int* __restrict__ corr,
                                                                       double* __restrict__ maha) {
   __shared__ __align__(16) unsigned char s_list[kRegWarps * kWarpListBytes];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -405,11 +407,11 @@ __global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv
   for (int i = blockIdx.x * kRegWarps + warp; i < n; i += gridDim.x * kRegWarps) {
     const float3 q = xform(Tf, __ldg(src + i));
     Neighbor nb;
-    const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, max_corr_sq, wl, nb);
+    const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, search_sq, wl, nb);
     const float d2 = __shfl_sync(kFull, nb.d2, 0);
     const int id = __shfl_sync(kFull, nb.id, 0);
     if (lane != 0) continue;
-    const int c = (nf > 0 && d2 < max_corr_sq) ? id : -1;
+    const int c = (nf > 0 && (double)d2 < max_corr_sq) ? id : -1;
     corr[i] = c;
     if (c >= 0) gicp_store_maha(src_nrm, tgt_nrm, i, c, T, maha);
   }
@@ -418,13 +420,14 @@ __global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv
 // update_correspondences, batched shape: one thread per source point (nn1_exact_thread)
 __global__ void __launch_bounds__(256) gicp_corr_thread_kernel(MapView mv, const float4* __restrict__ src, const double* __restrict__ src_nrm,
                                                                int n, const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
-                                                               float max_corr_sq, int* __restrict__ corr, double* __restrict__ maha) {
+                                                               float search_sq, double max_corr_sq, int* __restrict__ corr,
+                                                               double* __restrict__ maha) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float3 q = xform(Tf, __ldg(src + i));
   float d2; int id;
-  const bool f = nn1_exact_thread(mv, q.x, q.y, q.z, max_corr_sq, &d2, &id);
-  const int c = (f && d2 < max_corr_sq) ? id : -1;
+  const bool f = nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
+  const int c = (f && (double)d2 < max_corr_sq) ? id : -1;
   corr[i] = c;
   if (c >= 0) gicp_store_maha(src_nrm, tgt_nrm, i, c, T, maha);
 }
@@ -634,13 +637,14 @@ __device__ __forceinline__ float nn_scan_warp(const float4* __restrict__ tgt, in
 }
 
 // getFitnessScore (sum of squared 1-NN distances <= max_range, and their count) over block lb of the G blocks a cloud of n
-// points gets, stored as the block's row (sum, count) of partials.  WARP: one warp per point (knn_exact_warp), else one
+// points gets, stored as the block's row (sum, count) of partials.  As in the reference, the float d2 is compared with the
+// double max_range (PCL's `nn_dists[0] <= max_range`).  WARP: one warp per point (knn_exact_warp), else one
 // thread per point (nn1_exact_thread).  tgt != nullptr: points with no neighbour within search_sq get the exact one by a
 // scan of the whole target (nn_scan_*), for calc_fitness_score.  The single-pair kernel and the loop detector's batched
 // kernel (loop.cu) both run this body, so a candidate's row has the single-pair bits.
 template <bool WARP>
 __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* __restrict__ src, int n, int lb, int G, const Pose34f& Tf,
-                                              float search_sq, float max_range, const float4* __restrict__ tgt, int n_tgt,
+                                              float search_sq, double max_range, const float4* __restrict__ tgt, int n_tgt,
                                               double* __restrict__ partials) {
   __shared__ double s_acc[kRegWarps][2];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -655,7 +659,7 @@ __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* _
       float d2 = __shfl_sync(kFull, nb.d2, 0);
       bool found = nf > 0;
       if (!found && tgt) { d2 = nn_scan_warp(tgt, n_tgt, q.x, q.y, q.z); found = n_tgt > 0; }   // warp-uniform
-      if (found && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
+      if (found && (double)d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
     }
   } else {
     for (int i = lb * blockDim.x + threadIdx.x; i < n; i += G * blockDim.x) {
@@ -663,7 +667,7 @@ __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* _
       float d2; int id;
       bool found = nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
       if (!found && tgt) { d2 = nn_scan_thread(tgt, n_tgt, q.x, q.y, q.z); found = n_tgt > 0; }
-      if (found && d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
+      if (found && (double)d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
     }
     sum = warp_sum(sum); cnt = warp_sum(cnt);
   }
@@ -680,7 +684,7 @@ __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* _
 // shape asks for 3 blocks per SM, the thread shape for no minimum (0).
 template <bool WARP>
 __global__ void __launch_bounds__(kRegWarps * 32, WARP ? 3 : 0) fitness_kernel(MapView mv, const float4* __restrict__ src, int n,
-                                                                               Pose34f Tf, float search_sq, float max_range,
+                                                                               Pose34f Tf, float search_sq, double max_range,
                                                                                double* __restrict__ partials, unsigned* __restrict__ done,
                                                                                double* __restrict__ result, double seq, ShardComm sc) {
   fitness_range<WARP>(mv, src, n, (int)blockIdx.x, (int)gridDim.x, Tf, search_sq, max_range, nullptr, 0, partials);
@@ -741,9 +745,19 @@ constexpr int kThreadShapeMin = 16384;  // clouds from this size on use the thre
 static int reg_grid(int n) { return std::max(1, std::min((n + 255) / 256, kLioMaxGrid)); }
 static int warp_grid(int n) { return std::max(1, std::min((n + kRegWarps - 1) / kRegWarps, lsd::kNumSms * 6)); }
 
-// getFitnessScore's grid search radius: max_range, at most 64 map voxels
+// getFitnessScore's grid search radius: max_range, at most 64 map voxels.  Rounded to the nearest float, the bound holds every
+// float <= max_range (the nearest float is either the largest float <= max_range or above it).
 static float fitness_search_sq(double max_range, double map_resolution) {
   return (float)std::min(max_range, 64.0 * map_resolution * map_resolution * 64.0);
+}
+
+// The inclusive float bound of update_correspondences' grid search for the gate (double)d2 < max_corr_sq: max_corr_sq
+// rounded up to a float, so that it holds every float below max_corr_sq.  Squaring max_corr_dist in float instead can fall
+// below a float under the gate (max_corr_dist = 0.137) and lose that neighbour.  For a square that is a float, that float.
+static float corr_search_sq(double max_corr_sq) {
+  float f = (float)max_corr_sq;
+  if ((double)f < max_corr_sq) f = nextafterf(f, FLT_MAX);
+  return f;
 }
 
 // f(std::bool_constant<update>, std::bool_constant<deriv>): launches the <UPDATE, DERIV> instance of a cost kernel
@@ -800,13 +814,14 @@ static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H
     Pose34d Td; Pose34f Tf;
     T_to_pose(T, &Td, &Tf);
     if (update) {
-      const float mc = (float)r->p.max_corr_dist;
+      const double mc2 = r->p.max_corr_dist * r->p.max_corr_dist;
+      const float search = corr_search_sq(mc2);
       if (r->n_src >= kThreadShapeMin)
         gicp_corr_thread_kernel<<<(r->n_src + 255) / 256, 256, 0, st>>>(r->tgt_map->view, r->d_src, r->d_src_nrm, r->n_src, r->d_tgt_nrm, Td, Tf,
-                                                                        mc * mc, r->d_corr, r->d_maha);
+                                                                        search, mc2, r->d_corr, r->d_maha);
       else
         gicp_corr_kernel<<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->d_src_nrm, r->n_src, r->d_tgt_nrm, Td, Tf,
-                                                                       mc * mc, r->d_corr, r->d_maha);
+                                                                       search, mc2, r->d_corr, r->d_maha);
       r->launches++;
     }
     const int g = reg_grid(r->n_src);
@@ -1426,10 +1441,10 @@ lsd_status_t lsd_reg_fitness(lsd_reg_t* r, const double* T16_or_null, double max
   const double seq = (double)(++r->seq);
   const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
   if (r->n_src >= kThreadShapeMin)
-    fitness_kernel<false><<<reg_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, (float)max_range,
+    fitness_kernel<false><<<reg_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, max_range,
                                                                          r->d_partials, r->d_done, r->d_result, seq, r->sc);
   else
-    fitness_kernel<true><<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, (float)max_range,
+    fitness_kernel<true><<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, max_range,
                                                                         r->d_partials, r->d_done, r->d_result, seq, r->sc);
   LSD_CUDA(cudaGetLastError());
   r->launches++;

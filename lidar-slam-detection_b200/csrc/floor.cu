@@ -583,7 +583,7 @@ static lsd_status_t floor_run(lsd_floor* f, const float4* d_in, int n, lsd_floor
     float4* vg_out = f->d_inl;   // scratch until the inliers are written
     lsd_status_t s = vg_run(f->vg, d_in, n, P.prefilter_leaf, vg_out, f->d_counts, st);
     if (s) return s;
-    f->launches += 8;
+    f->launches += vg_launches(f->vg);
     src = vg_out; n_src = f->d_counts;
   }
   // 2. height clip (+ the distance filter) and the map insert of the clipped points

@@ -1282,7 +1282,7 @@ lsd_status_t lio_load(lsd_lio* l, const float4* d_scan, int n, int downsample) {
     lsd_status_t s = vg_run(l->vg, d_scan, n, l->p.filter_size_surf, l->d_body, l->d_n, st);
     if (s) return s;
     prof.stop();
-    l->launches += l->vg->input_order_sums ? 8 : 5;
+    l->launches += vg_launches(l->vg);
     l->n_bound = std::min(n, l->p.max_points);
     l->n_down = -1;  // learned with the first reduction (or lsd_lio_load_scan's explicit read)
   } else {
@@ -1322,7 +1322,7 @@ static lsd_status_t issue_side_vg(lsd_lio* l, lsd_lio::Stage* sg, const float4* 
   l->vg->pdl = (l->pdl && l->sc.world <= 1) ? 1 : 0;
   lsd_status_t s = vg_run(l->vg, src, sg->n, l->p.filter_size_surf, sg->body, sg->dn, l->copy_stream);
   if (s) return s;
-  l->launches += l->vg->input_order_sums ? 8 : 5;
+  l->launches += vg_launches(l->vg);
   LSD_CUDA(cudaEventRecord(sg->ev, l->copy_stream));
   LSD_CUDA(cudaEventRecord(l->ev_side_vg, l->copy_stream));
   l->side_vg_inflight = true;

@@ -15,7 +15,7 @@
 //
 // Pipeline (all sizes stay on the device, no host round trip):
 //   vg_minmax -> vg_mark (+grid setup) -> vg_scan (word scan; last block scans the chunk totals)
-//   -> vg_count -> vg_offsets -> vg_scatter -> vg_order -> vg_sum (+scratch cleanup)
+//   -> vg_count (+ the last block scans the per-leaf counts) -> vg_scatter -> vg_sum (+scratch cleanup)
 //   [fixed-point: -> vg_accum -> vg_finalize (+scratch cleanup)].  A single cooperative kernel with grid barriers
 //   was measured and rejected: no faster (the barriers cost what the launches do) and cooperative
 //   launches serialise badly behind an in-flight H2D copy (e2e 3.5 ms/scan vs 0.39 ms).
@@ -230,113 +230,219 @@ __global__ void __launch_bounds__(256) vg_finalize_kernel(const VgGrid* __restri
   }
 }
 
-// ---- the centroids as a sequential fp32 sum in INPUT order (kernels 4a-4e instead of 4 and 5) ----------------------------------
+// ---- the centroids as a sequential fp32 sum in INPUT order (kernels 4a-4c instead of 4 and 5) ----------------------------------
 // pcl::VoxelGrid adds a leaf's points one by one into fp32 accumulators, in the order std::sort leaves equal keys in, and divides
 // by the count; the restated filter the oracle and the reference arm use (oracle/lsd_oracle.c::orc_voxelgrid,
 // oracle/ref_shim_fastlio/pcl/filters/voxel_grid.h) fixes that order to the input order.  Reproducing THAT arithmetic — instead
 // of the exact fixed-point sums above, one fp32 ulp away for half the leaves — is what lets a whole scan agree with the
-// reference arm to the last bits of the double-precision sums (DESIGN.md section 4): a counting sort by leaf (count, exclusive
-// scan, scatter), the rank of every point inside its leaf's segment by counting smaller indices, then one thread per leaf
-// adding its points in that order.
+// reference arm to the last bits of the double-precision sums (DESIGN.md section 4): a counting sort by leaf (count + exclusive
+// scan of the counts, scatter), then every leaf sorts its members' input indices and adds its points in that order.  The scatter
+// leaves a leaf's members in arrival order, so the sort is what fixes the order of the additions.  Two size classes: a leaf of
+// at most kVgSmall points is one thread's (a sorting network in registers); a crowded one is a warp's (bitonic sort of the
+// indices in shared memory, the points gathered with all loads in flight, each channel one sequential fp32 chain); a big one
+// (more than kVgCap) is a block's (the sort in the block's shared memory, in place in global memory above kVgBig).
+constexpr int kVgSmall = 8;     // leaves of up to this many points: one thread each
+constexpr int kVgCap = 512;     // crowded leaves up to this many points: one warp each, sorting in its share of shared memory
+constexpr int kVgWarps = 8;     // warps per 256-thread block
+constexpr int kVgBig = kVgWarps * kVgCap;   // big leaves up to this many points sort in the whole block's shared memory
+constexpr int kVgTile = 2048;   // per-leaf counts per tile of vg_count_kernel's closing scan
+
 __global__ void __launch_bounds__(256) vg_count_kernel(const float4* __restrict__ in, int n, const VgGrid* __restrict__ gp,
                                                        const unsigned* __restrict__ bitmap, int* __restrict__ vidx,
                                                        const int* __restrict__ word_prefix, const int* __restrict__ chunk_off,
-                                                       int* __restrict__ cnt, int* __restrict__ out_vidx, float4* __restrict__ out) {
+                                                       int* __restrict__ cnt, int* __restrict__ slot, int* __restrict__ out_vidx,
+                                                       float4* __restrict__ out, const int* __restrict__ m_ptr, int* __restrict__ off,
+                                                       int* __restrict__ crowd, int* __restrict__ crowd_n, unsigned* __restrict__ done) {
   pdl_enter();
+  __shared__ int warp_tot[8];
+  __shared__ int carry, n_list, n_big;
+  __shared__ bool is_last;
+  __shared__ int tile[kVgTile];
   const int status = gp->status;
+  if (status) {
+    if (status == LSD_ERR_GRID_OVERFLOW)   // PCL: output = input
+      for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = __ldg(in + i);
+    return;
+  }
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    if (status == LSD_ERR_GRID_OVERFLOW) { out[i] = __ldg(in + i); continue; }  // PCL: output = input
-    if (status) return;
     const int idx = vidx[i];
     if (idx < 0) continue;   // non-finite point
     const int w = idx >> 5;
     const int rank = chunk_off[w / kScanChunk] + word_prefix[w] + __popc(bitmap[w] & ((1u << (idx & 31)) - 1u));
     vidx[i] = rank;          // from here on: the point's output slot
-    atomicAdd(cnt + rank, 1);
+    slot[i] = atomicAdd(cnt + rank, 1);   // and its place in the leaf's segment (arrival order)
     out_vidx[rank] = idx;
   }
-}
-// exclusive scan of the per-leaf counts: one block, every thread a contiguous run
-__global__ void __launch_bounds__(1024) vg_offsets_kernel(const VgGrid* __restrict__ gp, const int* __restrict__ m_ptr,
-                                                          const int* __restrict__ cnt, int* __restrict__ off) {
-  pdl_enter();
-  __shared__ int part[1024];
-  if (gp->status) return;
-  const int m = *m_ptr;
-  const int per = (m + 1023) / 1024, a = threadIdx.x * per, b = min(a + per, m);
-  int s = 0;
-  for (int r = a; r < b; r++) s += cnt[r];
-  part[threadIdx.x] = s;
+  // the last block to finish: exclusive scan of the per-leaf counts (off[m] = total) and the lists of crowded leaves (more than
+  // kVgSmall points, from the front of `crowd`) and of big leaves (more than kVgCap, from its back).  Tiles of kVgTile counts,
+  // read coalesced into shared memory, each thread then scanning a contiguous run of kVgTile / 256.
+  __threadfence();
   __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {
-    const int t = threadIdx.x >= o ? part[threadIdx.x - o] : 0;
+  if (threadIdx.x == 0) { is_last = atomicAdd(done, 1u) == gridDim.x - 1; carry = 0; n_list = 0; n_big = 0; }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  const int m = *m_ptr;
+  constexpr int per = kVgTile / 256;
+  for (int base = 0; base < m; base += kVgTile) {
+#pragma unroll
+    for (int u = 0; u < per; u++) { const int r = base + u * 256 + threadIdx.x; tile[u * 256 + threadIdx.x] = r < m ? __ldcg(cnt + r) : 0; }
     __syncthreads();
-    part[threadIdx.x] += t;
-    __syncthreads();
+    int v[per], s = 0;
+#pragma unroll
+    for (int u = 0; u < per; u++) { v[u] = tile[threadIdx.x * per + u]; s += v[u]; }
+    int incl;
+    int run = block_scan_step(s, warp_tot, &carry, &incl);   // ends with a barrier: the tile may be overwritten after it
+#pragma unroll
+    for (int u = 0; u < per; u++) {
+      const int r = base + threadIdx.x * per + u;
+      if (r < m) {
+        off[r] = run;
+        if (v[u] > kVgCap) crowd[m - 1 - atomicAdd(&n_big, 1)] = r;
+        else if (v[u] > kVgSmall) crowd[atomicAdd(&n_list, 1)] = r;
+      }
+      run += v[u];
+    }
   }
-  int run = part[threadIdx.x] - s;
-  for (int r = a; r < b; r++) { off[r] = run; run += cnt[r]; }
+  __syncthreads();
+  if (threadIdx.x == 0) { off[m] = carry; crowd_n[0] = n_list; crowd_n[1] = n_big; *done = 0u; }
 }
 __global__ void __launch_bounds__(256) vg_scatter_kernel(int n, const VgGrid* __restrict__ gp, const int* __restrict__ vidx,
-                                                         const int* __restrict__ off, int* __restrict__ cur, int* __restrict__ seg) {
+                                                         const int* __restrict__ slot, const int* __restrict__ off, int* __restrict__ seg) {
   pdl_enter();
   if (gp->status) return;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int r = vidx[i];
     if (r < 0) continue;
-    seg[off[r] + atomicAdd(cur + r, 1)] = i;
+    seg[off[r] + slot[i]] = i;
   }
 }
-__global__ void __launch_bounds__(256) vg_order_kernel(int n, const VgGrid* __restrict__ gp, const int* __restrict__ vidx,
-                                                       const int* __restrict__ off, const int* __restrict__ cnt,
-                                                       const int* __restrict__ seg, int* __restrict__ ord) {
-  pdl_enter();
-  if (gp->status) return;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int r = vidx[i];
-    if (r < 0) continue;
-    const int base = off[r], k = cnt[r];
-    int c = 0;
-#pragma unroll 8
-    for (int t = 0; t < k; t++) c += __ldcg(seg + base + t) < i ? 1 : 0;
-    ord[base + c] = i;
+
+// Ascending sort of s[0, n) by one warp (kBlock = false) or the whole block: bitonic with the first comparator of every merge
+// flipped, so that every comparator puts the smaller value first and positions >= n act as +infinity that never moves (their
+// comparators are skipped).
+template <bool kBlock, class T>
+__device__ __forceinline__ void sort_ids(T* s, int n) {
+  const int tid = kBlock ? (int)threadIdx.x : (int)(threadIdx.x & 31), nt = kBlock ? (int)blockDim.x : 32;
+  int lg = 0;
+  while ((1 << lg) < n) lg++;
+  const int pairs = (1 << lg) >> 1;
+  for (int lsz = 1; lsz <= lg; lsz++) {
+    for (int ls = lsz - 1; ls >= 0; ls--) {
+      for (int i = tid; i < pairs; i += nt) {
+        const int hi = (i >> ls) << (ls + 1), lo = i & ((1 << ls) - 1);
+        const int a = hi + lo, b = ls == lsz - 1 ? hi + (2 << ls) - 1 - lo : a + (1 << ls);
+        if (b < n) {
+          const int x = s[a], y = s[b];
+          if (x > y) { s[a] = y; s[b] = x; }
+        }
+      }
+      if (kBlock) __syncthreads(); else __syncwarp();
+    }
   }
 }
+
+// Sum of in[ids[0]], in[ids[1]], ... in that order, by one warp: 256 points requested at a time, then broadcast one by one;
+// every lane adds all four channels (the same sequential fp32 chains), lane 0's result is used.
+template <class T>
+__device__ __forceinline__ float4 warp_sum_in_order(const float4* __restrict__ in, T* ids, int k, int lane) {
+  float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
+  for (int t0 = 0; t0 < k; t0 += 32 * 8) {
+    float4 p[8];
+#pragma unroll
+    for (int u = 0; u < 8; u++) {
+      const int t = t0 + 32 * u + lane;
+      p[u] = t < k ? __ldg(in + ids[t]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int u = 0; u < 8; u++) {
+      const int nj = min(32, k - t0 - 32 * u);
+      for (int j = 0; j < nj; j++) {
+        ax += __shfl_sync(0xffffffffu, p[u].x, j);
+        ay += __shfl_sync(0xffffffffu, p[u].y, j);
+        az += __shfl_sync(0xffffffffu, p[u].z, j);
+        aw += __shfl_sync(0xffffffffu, p[u].w, j);
+      }
+    }
+  }
+  return make_float4(ax, ay, az, aw);
+}
+
+#define VG_CE(i, j) { const int lo_ = min(id[i], id[j]), hi_ = max(id[i], id[j]); id[i] = lo_; id[j] = hi_; }
+
+// One launch for all classes: blocks take the big leaves, warps the crowded ones, threads the rest (the last threads of the grid first,
+// so the warps busy with crowded leaves take none when there are fewer leaves than threads).  Every leaf writes only its own
+// output slot.  Scratch returns to its idle state: counts, bitmap words and bbox.
 __global__ void __launch_bounds__(256) vg_sum_kernel(const float4* __restrict__ in, const VgGrid* __restrict__ gp,
                                                      const int* __restrict__ m_ptr, const int* __restrict__ off, int* __restrict__ cnt,
-                                                     int* __restrict__ cur, const int* __restrict__ ord, const int* __restrict__ out_vidx,
-                                                     unsigned* __restrict__ bitmap, float4* __restrict__ out, int* __restrict__ bbox) {
+                                                     int* seg, const int* __restrict__ crowd, const int* __restrict__ crowd_n,
+                                                     const int* __restrict__ out_vidx, unsigned* __restrict__ bitmap,
+                                                     float4* __restrict__ out, int* __restrict__ bbox) {
   pdl_enter();
+  __shared__ int s_ids[kVgWarps][kVgCap];
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     bbox[0] = bbox[1] = bbox[2] = 0x7f7f7f7f;
     bbox[3] = bbox[4] = bbox[5] = (int)0x80808080;
   }
   if (gp->status) return;
-  const int m = *m_ptr;
-  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < m; r += gridDim.x * blockDim.x) {
-    const int base = off[r], k = cnt[r];
-    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
-    int t = 0;
-    for (; t + 8 <= k; t += 8) {     // eight members' indices, then their points, in flight together; the additions stay in input order
-      int id[8];
-      float4 p[8];
-#pragma unroll
-      for (int u = 0; u < 8; u++) id[u] = __ldcg(ord + base + t + u);
-#pragma unroll
-      for (int u = 0; u < 8; u++) p[u] = __ldg(in + id[u]);
-#pragma unroll
-      for (int u = 0; u < 8; u++) { ax += p[u].x; ay += p[u].y; az += p[u].z; aw += p[u].w; }
+  const int m = *m_ptr, n_crowd = crowd_n[0], n_big = crowd_n[1], lane = threadIdx.x & 31;
+  for (int j = blockIdx.x; j < n_big; j += gridDim.x) {   // big leaves: one block each, listed from the back of `crowd`
+    const int r = crowd[m - 1 - j], base = off[r], k = off[r + 1] - base;
+    int* sb = &s_ids[0][0];
+    if (k <= kVgBig) {
+      for (int t = threadIdx.x; t < k; t += blockDim.x) sb[t] = seg[base + t];
+      __syncthreads();
+      sort_ids<true>(sb, k);
+    } else {        // rare: sorted in place in global memory
+      sort_ids<true>(static_cast<volatile int*>(seg + base), k);
+      sb = nullptr;
     }
-    for (; t < k; t++) {
-      const float4 p = __ldg(in + __ldcg(ord + base + t));
-      ax += p.x; ay += p.y; az += p.z; aw += p.w;
+    if (threadIdx.x < 32) {
+      const float4 o = sb ? warp_sum_in_order(in, sb, k, lane) : warp_sum_in_order(in, static_cast<volatile int*>(seg + base), k, lane);
+      const float ck = (float)k;
+      if (lane == 0) out[r] = make_float4(o.x / ck, o.y / ck, o.z / ck, o.w / ck);
     }
-    const float c = (float)k;
-    out[r] = make_float4(ax / c, ay / c, az / c, aw / c);
-    cnt[r] = 0; cur[r] = 0;
+    __syncthreads();   // the sum has read the buffer before the next big leaf overwrites it
+  }
+  int* sid = s_ids[threadIdx.x >> 5];
+  for (int c = blockIdx.x * kVgWarps + (threadIdx.x >> 5); c < n_crowd; c += gridDim.x * kVgWarps) {   // crowded: one warp each
+    const int r = crowd[c], base = off[r], k = off[r + 1] - base;
+    for (int t = lane; t < k; t += 32) sid[t] = seg[base + t];
+    __syncwarp();
+    sort_ids<false>(sid, k);
+    const float4 o = warp_sum_in_order(in, sid, k, lane);
+    __syncwarp();   // every lane has read sid before the next leaf overwrites it
+    const float ck = (float)k;
+    if (lane == 0) out[r] = make_float4(o.x / ck, o.y / ck, o.z / ck, o.w / ck);
+  }
+  const int nt = gridDim.x * blockDim.x;
+  for (int r = nt - 1 - (int)(blockIdx.x * blockDim.x + threadIdx.x); r < m; r += nt) {
+    const int base = off[r], k = off[r + 1] - base;
+    cnt[r] = 0;
     bitmap[out_vidx[r] >> 5] = 0u;
+    if (k > kVgSmall) continue;
+    int id[kVgSmall];
+#pragma unroll
+    for (int u = 0; u < kVgSmall; u++) id[u] = u < k ? seg[base + u] : 0x7fffffff;
+    VG_CE(0, 2) VG_CE(1, 3) VG_CE(4, 6) VG_CE(5, 7)     // optimal 19-comparator network for 8 keys
+    VG_CE(0, 4) VG_CE(1, 5) VG_CE(2, 6) VG_CE(3, 7)
+    VG_CE(0, 1) VG_CE(2, 3) VG_CE(4, 5) VG_CE(6, 7)
+    VG_CE(2, 4) VG_CE(3, 5)
+    VG_CE(1, 4) VG_CE(3, 6)
+    VG_CE(1, 2) VG_CE(3, 4) VG_CE(5, 6)
+    float4 p[kVgSmall];
+#pragma unroll
+    for (int u = 0; u < kVgSmall; u++) p[u] = u < k ? __ldg(in + id[u]) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
+#pragma unroll
+    for (int u = 0; u < kVgSmall; u++)
+      if (u < k) { ax += p[u].x; ay += p[u].y; az += p[u].z; aw += p[u].w; }
+    const float ck = (float)k;
+    out[r] = make_float4(ax / ck, ay / ck, az / ck, aw / ck);
   }
 }
+#undef VG_CE
+static_assert(kVgSmall == 8, "vg_sum_kernel's sorting network is written for 8 keys");
 
 lsd_status_t vg_run(lsd_voxelgrid* g, const float4* d_in, int n, float leaf, float4* d_out, int* d_m, cudaStream_t st) {
   if (n > g->max_points) { set_error("voxelgrid: %d points exceed capacity %d", n, g->max_points); return LSD_ERR_CAPACITY; }
@@ -347,20 +453,20 @@ lsd_status_t vg_run(lsd_voxelgrid* g, const float4* d_in, int n, float leaf, flo
   LSD_LAUNCH(pdl, vg_mark_kernel, nb, 256, st, d_in, n, leaf, g->max_cells, g->bbox, g->grid, g->bitmap, g->vidx);
   LSD_LAUNCH(pdl, vg_scan_kernel, g->scan_blocks, 256, st, g->grid, g->bitmap, g->word_prefix, g->chunk_sum, g->done, d_m, n);
   if (g->input_order_sums) {
-    LSD_LAUNCH(pdl, vg_count_kernel, nb, 256, st, d_in, n, g->grid, g->bitmap, g->vidx, g->word_prefix, g->chunk_sum, g->cnt, g->out_vidx, d_out);
-    LSD_LAUNCH(pdl, vg_offsets_kernel, 1, 1024, st, g->grid, d_m, g->cnt, g->off);
-    LSD_LAUNCH(pdl, vg_scatter_kernel, nb, 256, st, n, g->grid, g->vidx, g->off, g->cur, g->seg);
-    LSD_LAUNCH(pdl, vg_order_kernel, nb, 256, st, n, g->grid, g->vidx, g->off, g->cnt, g->seg, g->ord);
-    LSD_LAUNCH(pdl, vg_sum_kernel, nb, 256, st, d_in, g->grid, d_m, g->off, g->cnt, g->cur, g->ord, g->out_vidx, g->bitmap, d_out, g->bbox);
+    LSD_LAUNCH(pdl, vg_count_kernel, nb, 256, st, d_in, n, g->grid, g->bitmap, g->vidx, g->word_prefix, g->chunk_sum, g->cnt, g->slot,
+               g->out_vidx, d_out, d_m, g->off, g->crowd, g->crowd_n, g->done + 1);
+    LSD_LAUNCH(pdl, vg_scatter_kernel, nb, 256, st, n, g->grid, g->vidx, g->slot, g->off, g->seg);
+    LSD_LAUNCH(pdl, vg_sum_kernel, nb, 256, st, d_in, g->grid, d_m, g->off, g->cnt, g->seg, g->crowd, g->crowd_n, g->out_vidx, g->bitmap,
+               d_out, g->bbox);
     LSD_CUDA(cudaGetLastError());
-    g->launches += 8;
+    g->launches += vg_launches(g);
     return LSD_OK;
   }
   LSD_LAUNCH(pdl, vg_accum_kernel, nb, 256, st, d_in, n, g->grid, g->bitmap, g->vidx, g->word_prefix, g->chunk_sum, g->sums, g->cnt,
              g->out_vidx, d_out);
   LSD_LAUNCH(pdl, vg_finalize_kernel, nb, 256, st, g->grid, d_m, g->sums, g->cnt, g->out_vidx, g->bitmap, d_out, g->bbox);
   LSD_CUDA(cudaGetLastError());
-  g->launches += 5;
+  g->launches += vg_launches(g);
   return LSD_OK;
 }
 
@@ -392,10 +498,11 @@ lsd_status_t lsd_voxelgrid_create(lsd_voxelgrid_t** out, int max_points, int log
   A((void**)&g->out_vidx, (size_t)max_points * 4);
   A((void**)&g->sums, (size_t)max_points * 4 * 8);
   A((void**)&g->cnt, (size_t)max_points * 4);
-  A((void**)&g->off, (size_t)max_points * 4);
-  A((void**)&g->cur, (size_t)max_points * 4);
+  A((void**)&g->off, ((size_t)max_points + 1) * 4);
+  A((void**)&g->slot, (size_t)max_points * 4);
   A((void**)&g->seg, (size_t)max_points * 4);
-  A((void**)&g->ord, (size_t)max_points * 4);
+  A((void**)&g->crowd, (size_t)max_points * 4);
+  A((void**)&g->crowd_n, 64);
   { const char* ev = getenv("LSD_VG_SUMS"); g->input_order_sums = (ev && ev[0] == 'f') ? 0 : 1; }   // "fixed": the exact fixed-point sums
   A((void**)&g->io_in, (size_t)max_points * 16);
   A((void**)&g->io_out, (size_t)max_points * 16);
@@ -414,7 +521,7 @@ lsd_status_t lsd_voxelgrid_destroy(lsd_voxelgrid_t* g) {
   cudaSetDevice(g->device);
   if (g->stream) cudaStreamSynchronize(g->stream);
   void* ptrs[] = {g->bbox, g->grid, g->bitmap, g->word_prefix, g->chunk_sum, g->vidx, g->out_vidx, g->sums, g->cnt, g->io_in, g->io_out, g->d_m, g->done,
-                  g->off, g->cur, g->seg, g->ord};
+                  g->off, g->slot, g->seg, g->crowd, g->crowd_n};
   for (void* p : ptrs) cudaFree(p);
   if (g->stream) cudaStreamDestroy(g->stream);
   delete g;

@@ -26,15 +26,17 @@ struct lsd_voxelgrid {
   int* out_vidx = nullptr;        // leaf index per output point
   long long* sums = nullptr;      // [max_points,4] fixed-point channel sums; all-zero between calls
   int* cnt = nullptr;
-  int *off = nullptr, *cur = nullptr, *seg = nullptr, *ord = nullptr;   // input-order sums: leaf offsets, scatter cursors (zero between calls), members, members in input order
+  int *off = nullptr, *slot = nullptr, *seg = nullptr;   // input-order sums: leaf offsets [m+1], each point's place in its leaf's segment, members
+  int *crowd = nullptr, *crowd_n = nullptr;               // crowded leaves (front) and big leaves (back) and their numbers (written by every call)
   int input_order_sums = 1;       // centroids as pcl::VoxelGrid's sequential fp32 sums in input order (LSD_VG_SUMS=fixed: exact fixed-point sums)
   float4 *io_in = nullptr, *io_out = nullptr;  // staging for the host-pointer entry point
   int* d_m = nullptr;
-  unsigned* done = nullptr;       // last-block ticket of vg_scan_kernel
+  unsigned* done = nullptr;       // last-block tickets: [0] vg_scan_kernel, [1] vg_count_kernel
   long long launches = 0;
-  int pdl = 0;                    // launch the five kernels with programmatic dependent launch (lsd_lio_set_pdl)
+  int pdl = 0;                    // launch the kernels with programmatic dependent launch (lsd_lio_set_pdl)
 };
 
 namespace lsd {
 lsd_status_t vg_run(lsd_voxelgrid* g, const float4* d_in, int n, float leaf, float4* d_out, int* d_m, cudaStream_t st);
+inline int vg_launches(const lsd_voxelgrid* g) { return g->input_order_sums ? 6 : 5; }   // kernels per vg_run with n > 0
 }

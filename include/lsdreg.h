@@ -229,6 +229,10 @@ lsd_status_t lsd_lio_reference_order_fallbacks(lsd_lio_t* l, unsigned* count);
  * path_out (optional): 1 = warp-cooperative replay, 2 = it left at introselect's depth limit and the serial replay took over,
  * 3 = serial replay (n > 32). */
 lsd_status_t lsd_debug_nth_element(const float* dist_host, int n, int first, int nth, int last, int* perm_out_host, int* path_out_host);
+/* Test entry: the LIO search's plane fit (esti_plane, common_lib.h:236-268) alone, one device thread per set.  pts5_host
+ * [n,5,3] (host), thr the residual threshold; pabcd_out [n,4] the plane (a, b, c, d), ok_out [n] 1 where every point is
+ * within thr of it. */
+lsd_status_t lsd_debug_esti_plane(const float* pts5_host, int n, float thr, float* pabcd_out, int* ok_out);
 /* Shape of the per-scan neighbour search (no reference counterpart): 0 or 1 = one warp per scan point (the only shape;
  * the flat shapes of round 1 were retired). */
 lsd_status_t lsd_lio_set_knn_shape(lsd_lio_t* l, int shape);

@@ -161,6 +161,7 @@ SIGNATURES = [
     ("lsd_lio_set_reference_order", _i, [_vp, _i]),
     ("lsd_lio_reference_order_fallbacks", _i, [_vp, _vp]),
     ("lsd_debug_nth_element", _i, [_vp, _i, _i, _i, _i, _vp, _vp]),
+    ("lsd_debug_esti_plane", _i, [_vp, _i, _f, _vp, _vp]),
     ("lsd_lio_set_knn_shape", _i, [_vp, _i]),
     ("lsd_lio_set_pdl", _i, [_vp, _i]),
     ("lsd_lio_shard_exchange_stats", _i, [_vp, C.POINTER(_d), C.POINTER(C.c_longlong)]),
@@ -493,6 +494,17 @@ def debug_nth_element(dist: np.ndarray, first: int, nth: int, last: int):
     path = C.c_int()
     check(lib.lsd_debug_nth_element(_ptr(d), d.shape[0], first, nth, last, _ptr(perm), C.byref(path)))
     return perm, path.value
+
+
+def debug_esti_plane(pts5: np.ndarray, thr: float = 0.1):
+    """The LIO search's plane fit on the device, one thread per 5-point set (include/lsdreg.h lsd_debug_esti_plane)
+    -> (pabcd [n,4] float32, ok [n] int32)."""
+    p = np.ascontiguousarray(pts5, np.float32).reshape(-1, 5, 3)
+    n = p.shape[0]
+    pabcd = np.empty((n, 4), np.float32)
+    ok = np.empty(n, np.int32)
+    check(lib.lsd_debug_esti_plane(_ptr(p), n, thr, _ptr(pabcd), _ptr(ok)))
+    return pabcd, ok
 
 
 def state_boxplus(x: np.ndarray, d: np.ndarray) -> np.ndarray:

@@ -1662,6 +1662,40 @@ lsd_status_t lsd_debug_nth_element(const float* dist_host, int n, int first, int
   if (path_out_host) *path_out_host = path;
   return LSD_OK;
 }
+// Test entry: esti_plane_dev — the function lio_hmodel_kernel<true> calls — on arbitrary 5-point sets, one thread per set.
+__global__ void __launch_bounds__(256) debug_esti_plane_kernel(const float* __restrict__ pts5, int n, float thr, float4* __restrict__ pabcd_out,
+                                                               int* __restrict__ ok_out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float px[5], py[5], pz[5];
+#pragma unroll
+  for (int j = 0; j < 5; j++) { px[j] = pts5[(size_t)i * 15 + 3 * j]; py[j] = pts5[(size_t)i * 15 + 3 * j + 1]; pz[j] = pts5[(size_t)i * 15 + 3 * j + 2]; }
+  float pabcd[4];
+  const bool ok = esti_plane_dev(px, py, pz, thr, pabcd);
+  pabcd_out[i] = make_float4(pabcd[0], pabcd[1], pabcd[2], pabcd[3]);
+  ok_out[i] = ok ? 1 : 0;
+}
+lsd_status_t lsd_debug_esti_plane(const float* pts5_host, int n, float thr, float* pabcd_out, int* ok_out) {
+  if (n < 0 || (n > 0 && (!pts5_host || !pabcd_out || !ok_out))) return LSD_ERR_INVALID;
+  if (n == 0) return LSD_OK;
+  lsd_status_t s = ensure_device();
+  if (s) return s;
+  float* d = nullptr; float4* p = nullptr; int* o = nullptr;
+  cudaError_t e = cudaMalloc((void**)&d, (size_t)n * 60);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&p, (size_t)n * 16);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&o, (size_t)n * 4);
+  if (e == cudaSuccess) e = cudaMemcpy(d, pts5_host, (size_t)n * 60, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) {
+    debug_esti_plane_kernel<<<(n + 255) / 256, 256>>>(d, n, thr, p, o);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = cudaMemcpy(pabcd_out, p, (size_t)n * 16, cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(ok_out, o, (size_t)n * 4, cudaMemcpyDeviceToHost);
+  cudaFree(d); cudaFree(p); cudaFree(o);
+  if (e != cudaSuccess) return cuda_fail(e, "lsd_debug_esti_plane", __FILE__, __LINE__);
+  return LSD_OK;
+}
 // -> queries since the handle's creation whose candidates overflowed the search's list (answered in canonical order)
 lsd_status_t lsd_lio_reference_order_fallbacks(lsd_lio_t* l, unsigned* count) {
   if (!l || !count) return LSD_ERR_INVALID;

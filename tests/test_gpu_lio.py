@@ -88,9 +88,12 @@ def test_update_pose_parity_and_map_incremental(small_world, literal, ref_order)
     np.testing.assert_allclose(Pg, o.P, rtol=1e-4, atol=1e-12)  # literal and Schur forms both
     # converged onto the ground truth (scan noise 2 cm)
     assert np.abs(xg[0:3] - small_world["tgt"]).max() < 0.02
-    # map_incremental: same add / skip decisions, same resulting map
+    # map_incremental: same add / skip decision for every point, same resulting map
     added_o = o.map_incremental(body)
     added_g = g.map_incremental(xo)  # same state on both sides
+    flags, _ = g.get_map_flags()
+    bad = np.nonzero(flags != o.flags)[0]
+    assert not len(bad), f"map_incremental flags differ at {bad[:8]}: {flags[bad[:8]]} vs {o.flags[bad[:8]]}"
     assert added_g == added_o
     st = g.map.stats()
     assert st["points"] == o.map.num_points and st["cells"] == o.map.num_cells

@@ -68,7 +68,8 @@ lsd_status_t lsd_map_create(lsd_map_t** out, float resolution, int log2_lines);
 lsd_status_t lsd_map_destroy(lsd_map_t* m);
 lsd_status_t lsd_map_clear(lsd_map_t* m);
 /* Tile sharding (SURVEY.md §8e): the map keeps only points in x-y tiles (tile_cells voxels wide) this
- * rank owns, plus a halo of reach_cells voxels; queries are answered from the local shard. */
+ * rank owns, plus a halo of reach_cells voxels; queries are answered from the local shard, and lsd_knn_query(_dev) on
+ * a sharded map refuses a stencil reaching further than the halo (EXACT: ceil(sqrt(max_sq)/res)+1 voxels). */
 lsd_status_t lsd_map_set_shard(lsd_map_t* m, int rank, int world, int tile_cells, int reach_cells);
 /* IVox::AddPoints.  Point i is stored with id = id0 + i (ids are what k-NN queries return). */
 lsd_status_t lsd_map_insert(lsd_map_t* m, const float* xyzi_host, int n, int32_t id0);
@@ -257,7 +258,10 @@ lsd_status_t lsd_lio_set_next_id(lsd_lio_t* l, int32_t id); /* flg_EKF_inited, l
  *   1. every rank: lsd_lio_shard_export(l, rank, world, tile_cells, reach_cells, blob)   (<= 8 ranks)
  *   2. all-gather the LSD_SHARD_BLOB_BYTES blobs (torch.distributed / MPI / a pipe)
  *   3. every rank: lsd_lio_shard_connect(l, blobs[world])
- * reach_cells: 1 for NEARBY6/18/26, 2 for NEARBY74, ceil(sqrt(5)/res)+1 for the exact search. */
+ * reach_cells: 1 for NEARBY6/18/26, 2 for NEARBY74, ceil(sqrt(5)/res)+1 for the exact search (6 at res 0.5); tile_cells
+ * must exceed 2 * reach_cells.  Enforced: with world > 1, lsd_lio_shard_export refuses (LSD_ERR_INVALID) a reach_cells
+ * below what the handle's search needs, and lsd_lio_set_nearby refuses a stencil the exported halo cannot serve —
+ * a narrower halo would not fail, it would silently drop neighbours of queries near a tile border. */
 #define LSD_SHARD_BLOB_BYTES 192
 lsd_status_t lsd_lio_shard_export(lsd_lio_t* l, int rank, int world, int tile_cells, int reach_cells, unsigned char* blob_out);
 lsd_status_t lsd_lio_shard_connect(lsd_lio_t* l, const unsigned char* blobs);

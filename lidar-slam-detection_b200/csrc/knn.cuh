@@ -21,6 +21,13 @@ __host__ __device__ __forceinline__ int stencil_slot(int type) {
   return type == LSD_STENCIL_CENTER ? 0 : type == LSD_STENCIL_NEARBY6 ? 1 : type == LSD_STENCIL_NEARBY18 ? 2
        : type == LSD_STENCIL_NEARBY26 ? 3 : type == LSD_STENCIL_NEARBY74 ? 4 : -1;
 }
+// How far (voxels, Chebyshev in x-y) a search with this stencil reaches from the query's home voxel: the halo a tile-sharded
+// map needs so that every voxel an owned query probes is held locally.  EXACT: knn_exact_warp's last shell.  -1: unknown.
+__host__ __device__ __forceinline__ int stencil_reach(int type, float max_sq, float inv_res) {
+  if (type == LSD_STENCIL_EXACT) return (int)ceilf(sqrtf(max_sq) * inv_res) + 1;
+  const int s = stencil_slot(type);
+  return s < 0 ? -1 : s == 0 ? 0 : s == 4 ? 2 : 1;
+}
 
 constexpr unsigned kFull = 0xffffffffu;
 constexpr int kCandCap = 256;  // per-warp candidate list capacity (one 32-cell chunk adds <= 224)

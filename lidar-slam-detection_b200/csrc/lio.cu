@@ -1037,8 +1037,10 @@ lsd_status_t lio_linearize(lsd_lio* l, const double* x, bool search, double* HTH
   const int pdl = l->pdl && l->sc.world <= 1;   // programmatic dependent launch (lsd_lio_set_pdl); single-GPU chains only
   ProfScope prof(l, search ? 0 : 1);
   if (search) {
-    const int keep_stale = (l->stale_rows && !l->p.knn_mode_exact && l->map->view.shard_world <= 1) ? 1 : 0;
-    const int ref_order = (l->reference_order && !l->p.knn_mode_exact && l->d_ref_fallbacks) ? 1 : 0;
+    // iVox stencils only: the exact search (knn_mode_exact, or lsd_lio_set_nearby(LSD_STENCIL_EXACT)) clears its output and
+    // returns sorted neighbours
+    const int keep_stale = (l->stale_rows && stencil != LSD_STENCIL_EXACT && l->map->view.shard_world <= 1) ? 1 : 0;
+    const int ref_order = (l->reference_order && stencil != LSD_STENCIL_EXACT && l->d_ref_fallbacks) ? 1 : 0;
     int resize_parity = -1;
     if (l->rows_resize_pending) { resize_parity = l->rows_parity; l->rows_parity ^= 1; l->rows_resize_pending = false; }
     const int nb = std::max(1, std::min((l->n_bound + kHmWarps - 1) / kHmWarps, l->max_search_blocks));
@@ -1734,8 +1736,18 @@ lsd_status_t lsd_lio_set_knn_shape(lsd_lio_t* l, int shape) {
   l->knn_shape = shape;
   return LSD_OK;
 }
+// Halo (voxels) the handle's per-scan search needs on a tile-sharded map: lio_linearize's stencil at its 5 m^2 radius.
+static int lio_search_reach(const lsd_lio* l, int nearby) {
+  return stencil_reach(l->p.knn_mode_exact ? LSD_STENCIL_EXACT : nearby, 5.0f, l->map->view.inv_res);
+}
 lsd_status_t lsd_lio_set_nearby(lsd_lio_t* l, int stencil) {
   if (!l || (stencil != LSD_STENCIL_EXACT && stencil_slot(stencil) < 0)) return LSD_ERR_INVALID;
+  const MapView& mv = l->map->view;
+  if (mv.shard_world > 1 && lio_search_reach(l, stencil) > mv.shard_reach) {
+    set_error("lsd_lio_set_nearby: stencil %d reaches %d voxels, the tile-sharded map's halo only %d (export with a wider reach_cells)",
+              stencil, lio_search_reach(l, stencil), mv.shard_reach);
+    return LSD_ERR_INVALID;
+  }
   l->p.ivox_nearby = stencil;
   return LSD_OK;
 }
@@ -1750,6 +1762,12 @@ static_assert(sizeof(ShardBlob) <= LSD_SHARD_BLOB_BYTES, "LSD_SHARD_BLOB_BYTES t
 
 lsd_status_t lsd_lio_shard_export(lsd_lio_t* l, int rank, int world, int tile_cells, int reach_cells, unsigned char* blob_out) {
   if (!l || !blob_out || world < 1 || world > kMaxRanks || rank < 0 || rank >= world) { set_error("lsd_lio_shard_export: bad rank/world (max %d ranks)", kMaxRanks); return LSD_ERR_INVALID; }
+  if (world > 1 && reach_cells < lio_search_reach(l, l->p.ivox_nearby)) {
+    // a narrower halo does not fail later: owned queries near a tile border would silently lose neighbours
+    set_error("lsd_lio_shard_export: the handle's search reaches %d voxels (%s), reach_cells %d is too narrow", lio_search_reach(l, l->p.ivox_nearby),
+              l->p.knn_mode_exact ? "exact search" : "iVox stencil", reach_cells);
+    return LSD_ERR_INVALID;
+  }
   LSD_CUDA(cudaSetDevice(l->device));
   lsd_status_t s = lsd_map_set_shard(l->map, rank, world, tile_cells, reach_cells);
   if (s) return s;

@@ -535,6 +535,12 @@ lsd_status_t launch_knn(lsd_map* m, const float4* d_q, int nq, int k, float max_
                         int* d_cnt, cudaStream_t st) {
   if (nq <= 0) return LSD_OK;
   if (stencil != LSD_STENCIL_EXACT && stencil_slot(stencil) < 0) { set_error("unknown stencil %d", stencil); return LSD_ERR_INVALID; }
+  if (m->view.shard_world > 1 && stencil_reach(stencil, max_sq, m->view.inv_res) > m->view.shard_reach) {
+    // a wider search than the halo would silently miss the neighbours in voxels this shard does not hold
+    set_error("k-NN on a tile-sharded map: stencil %d reaches %d voxels, the shard's halo only %d", stencil,
+              stencil_reach(stencil, max_sq, m->view.inv_res), m->view.shard_reach);
+    return LSD_ERR_INVALID;
+  }
   const int shape = m->knn_shape;  // 0 auto, 1 warp/query, 2 thread/query, 3 brick pages (lsd_knn_set_shape)
   {
     // brick pages: fixed stencils of reach 1 (CENTER / NEARBY6 / 18 / 26), k in {1, 5}; auto from kThreadKnnMin queries on

@@ -9,7 +9,19 @@ from __future__ import annotations
 import numpy as np
 
 TILE_CELLS = 32   # 16 m tiles at 0.5 m voxels: ~40 tiles per 120 x 80 m block, 13 % halo at reach 1
-REACH = {0: 1, 6: 1, 18: 1, 26: 1, 74: 2}
+REACH = {0: 1, 6: 1, 18: 1, 26: 1, 74: 2}   # iVox stencil -> halo (voxels) its search needs; the exact search: exact_reach
+STENCIL_EXACT = 1000
+
+
+def exact_reach(res: float = 0.5, max_sq: float = 5.0) -> int:
+    """Halo (voxels) the exact search needs: its last shell, ceil(sqrt(max_sq) / res) + 1, in the device's fp32 (6 at 0.5 m)."""
+    inv = np.float32(1.0 / np.float64(np.float32(res)))
+    return int(np.ceil(np.sqrt(np.float32(max_sq)) * inv)) + 1
+
+
+def reach_for(stencil: int, res: float = 0.5) -> int:
+    """reach_cells to export for a handle searching with `stencil` (STENCIL_EXACT for knn_mode_exact = 1)."""
+    return exact_reach(res) if stencil == STENCIL_EXACT else REACH[stencil]
 
 
 def cell_of(xyz: np.ndarray, res: float = 0.5) -> np.ndarray:
@@ -43,7 +55,11 @@ def relevant(cells: np.ndarray, rank: int, world: int, tile: int = TILE_CELLS, r
 
 
 def connect(lio, rank: int, world: int, group=None, tile_cells: int = TILE_CELLS, reach_cells: int = 1):
-    """Exchange the shard blobs over torch.distributed and connect `lio` to its peers."""
+    """Exchange the shard blobs over torch.distributed and connect `lio` to its peers.
+
+    reach_cells must cover the handle's search: `reach_for(ivox_nearby)` — 1 for NEARBY6/18/26, 2 for NEARBY74 — or
+    `exact_reach(ivox_resolution)` with knn_mode_exact = 1, and tile_cells must exceed 2 * reach_cells.  The export refuses
+    a narrower halo (LsdError), as does a later set_nearby to a wider stencil."""
     import torch
     import torch.distributed as dist
     blob = lio.shard_export(rank, world, tile_cells, reach_cells)

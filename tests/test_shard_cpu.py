@@ -32,6 +32,55 @@ def test_ownership_is_a_partition_and_halo_covers_the_stencil():
         assert balance.max() < 2.0 / world + 0.05
 
 
+def _tile_owner_scalar(cx, cy, tile, world):
+    """csrc/lsd_common.cuh::tile_owner in Python integers: floor division, 32-bit unsigned hash arithmetic."""
+    m = 0xFFFFFFFF
+    tx, ty = (cx // tile) & m, (cy // tile) & m
+    h = ((tx * 73856093) & m) ^ ((ty * 19349663) & m)
+    h ^= h >> 15
+    h = (h * 0x2C1B3C6D) & m
+    h ^= h >> 12
+    return h % world
+
+
+@pytest.mark.parametrize("reach", [1, 2, 6])
+def test_host_mirror_against_brute_force(reach):
+    """shard.tile_owner / owns / relevant against their definitions, cell by cell over [-3 tile, 3 tile]^2 (around 0, where
+    floor division and truncation differ): relevant(c, r) <=> some voxel within Chebyshev distance `reach` of c in x-y is
+    owned by r.  The four-corner test of shard_relevant is only right for tile >= 2 reach + 1 (a tile then spans the whole
+    window, so the window's tiles are those of its corners); this is its check at the bound and above it."""
+    for tile in (2 * reach + 1, 2 * reach + 2, 3 * reach + 4):
+        span = np.arange(-3 * tile, 3 * tile + 1)
+        cx, cy = np.meshgrid(span, span, indexing="ij")
+        cells = np.stack([cx.ravel(), cy.ravel(), np.zeros(cx.size, np.int64)], 1).astype(np.int32)
+        pad = np.arange(-3 * tile - reach, 3 * tile + reach + 1)
+        for world in (2, 3, 5):
+            own_tab = np.array([[_tile_owner_scalar(int(x), int(y), tile, world) for y in pad] for x in pad])
+            got = shard.tile_owner(np.repeat(pad, pad.size), np.tile(pad, pad.size), tile, world).reshape(pad.size, pad.size)
+            assert np.array_equal(got, own_tab), (tile, world)
+            o = reach                                        # index of span[0] in pad is reach
+            for r in range(world):
+                mine = own_tab == r
+                # brute force: any owned cell in the (2 reach + 1)^2 window
+                win = np.zeros((span.size, span.size), bool)
+                for dx in range(-reach, reach + 1):
+                    for dy in range(-reach, reach + 1):
+                        win |= mine[o + dx:o + dx + span.size, o + dy:o + dy + span.size]
+                rel = shard.relevant(cells, r, world, tile, reach).reshape(span.size, span.size)
+                assert np.array_equal(rel, win), (tile, world, r, np.argwhere(rel != win)[:4])
+                assert np.array_equal(shard.owns(cells, r, world, tile).reshape(span.size, span.size), mine[o:-o, o:-o])
+            # every cell owned by exactly one rank; negative tiles differ from the positive ones they would truncate to
+            assert (sum((own_tab == r).astype(int) for r in range(world)) == 1).all()
+        assert any(_tile_owner_scalar(-1, 0, tile, w) != _tile_owner_scalar(0, 0, tile, w) for w in (2, 3, 5))
+
+
+def test_exact_search_reach():
+    """The halo the exact search needs: its last shell ceil(sqrt(max_sq) / res) + 1 (csrc/knn.cuh::knn_exact_warp)."""
+    assert shard.exact_reach(0.5) == 6 and shard.exact_reach(1.0) == 4 and shard.exact_reach(0.25) == 10
+    assert shard.reach_for(shard.STENCIL_EXACT, 0.5) == 6
+    assert [shard.reach_for(s) for s in (0, 6, 18, 26, 74)] == [1, 1, 1, 1, 2]
+
+
 def _worker(rank, world, port, q):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)

@@ -582,6 +582,19 @@ lsd_status_t lsd_galign_cost(lsd_galign_t* h, int32_t new_slot, int32_t ref_slot
  * 225-255: hash voxelisation, <= max_points_per_voxel points per voxel, mean -> fp16).  Output rows are in
  * order of each voxel's first point; features [V, num_feature] fp16, indices [V,4] u32 = (0, z, y, x) or
  * (0, x, y, z).  The closed libspconv engine that consumes them is out of scope (SURVEY F5).
+ * The window keeps the reference's counts: a realtime frame gets at least one row even when the other frames fill
+ * max_points, so the total (and lsd_vfe_get_points) can reach max_points + max_frame_num - 1 rows.  A NaN coordinate
+ * passes the range test and lands in cell 0 of its axis, as in the reference.  Deviations from the reference:
+ *   - an empty realtime frame (num_points = 0, points_host may be NULL) reads nothing from the caller; the one row the
+ *     reference counts for it (and copies from the caller's array) is written as (1e30, 1e30, 1e30, 0, ...), which no
+ *     rigid motion brings into a range box;
+ *   - the window transform carries every feature past z and adds 0.1 to feature 4 only when num_feature > 4 (the
+ *     reference copies features 3 and 4 whatever num_feature is);
+ *   - a cell that only the range test rejects (a max face inside a grid rounded up) yields no row; the reference emits a
+ *     row of NaN features for it;
+ *   - realtime = 0 empties every frame slot (the reference's resize keeps the older slots' counts, so its next realtime
+ *     frame subtracts rows that are no longer in the window);
+ *   - lsd_vfe_create returns LSD_ERR_INVALID for a grid of 2^31 cells or more (voxel keys are 32-bit).
  * ------------------------------------------------------------------------------------------ */
 typedef struct lsd_vfe lsd_vfe_t;
 typedef struct lsd_vfe_params {

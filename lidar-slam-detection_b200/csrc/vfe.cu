@@ -13,6 +13,8 @@
 // (:229-232) and no host synchronisation between the passes (:248).
 #include <cuda_fp16.h>
 
+#include <climits>
+
 #include "lsd_common.cuh"
 
 namespace lsd {
@@ -31,7 +33,8 @@ __device__ __forceinline__ unsigned vfe_hash(unsigned k) {  // murmur3 fmix32, v
 // transform_kernel (preprocess_kernel.cu:6-20): older frames re-projected by the 3x4 motion, time + 0.1.
 // The reference is compiled with nvcc's default FMA contraction; its SASS for m0*x + m1*y + m2*z + m3 is
 // FMUL m1*y; FFMA m0*x + .; FFMA m2*z + .; FADD m3 — spelt out so this build (-fmad=false) produces the same bits
-// (pinned against the recompiled reference kernel, tests/test_gpu_ref_cuda.py).
+// (pinned against the recompiled reference kernel, tests/test_gpu_ref_cuda.py).  Features past z are carried over and
+// the time channel (feature 4) gets + 0.1; the reference copies features 3 and 4 whatever num_feature is.
 __global__ void __launch_bounds__(256) vfe_transform_kernel(int n, const float* __restrict__ src, float* __restrict__ dst, int nf,
                                                             const float* __restrict__ m) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -40,13 +43,18 @@ __global__ void __launch_bounds__(256) vfe_transform_kernel(int n, const float* 
   dst[nf * i + 0] = __fadd_rn(__fmaf_rn(m[2], pz, __fmaf_rn(m[0], px, __fmul_rn(m[1], py))), m[3]);
   dst[nf * i + 1] = __fadd_rn(__fmaf_rn(m[6], pz, __fmaf_rn(m[4], px, __fmul_rn(m[5], py))), m[7]);
   dst[nf * i + 2] = __fadd_rn(__fmaf_rn(m[10], pz, __fmaf_rn(m[8], px, __fmul_rn(m[9], py))), m[11]);
-  dst[nf * i + 3] = src[nf * i + 3];
-  dst[nf * i + 4] = (float)((double)src[nf * i + 4] + 0.1);
+  for (int f = 3; f < nf; f++) dst[nf * i + f] = f == 4 ? (float)((double)src[nf * i + 4] + 0.1) : src[nf * i + f];
+}
+
+// floor((p - mn) / vs) as an int; NaN gives 0, as the reference's float-to-int conversion on the device does
+__device__ __forceinline__ int vfe_cell(float p, float mn, float vs) {
+  const float c = floorf((p - mn) / vs);
+  return c == c ? (int)c : 0;
 }
 
 __device__ __forceinline__ unsigned vfe_voxel_offset(const VfeGrid& g, float px, float py, float pz, int* ix, int* iy, int* iz) {
-  if (px < g.mn[0] || px >= g.mx[0] || py < g.mn[1] || py >= g.mx[1] || pz < g.mn[2] || pz >= g.mx[2]) return kVfeEmpty;
-  const int x = (int)floorf((px - g.mn[0]) / g.vs[0]), y = (int)floorf((py - g.mn[1]) / g.vs[1]), z = (int)floorf((pz - g.mn[2]) / g.vs[2]);
+  if (px < g.mn[0] || px >= g.mx[0] || py < g.mn[1] || py >= g.mx[1] || pz < g.mn[2] || pz >= g.mx[2]) return kVfeEmpty;  // NaN passes
+  const int x = vfe_cell(px, g.mn[0], g.vs[0]), y = vfe_cell(py, g.mn[1], g.vs[1]), z = vfe_cell(pz, g.mn[2], g.vs[2]);
   if (x < 0 || x >= g.gs[0] || y < 0 || y >= g.gs[1] || z < 0 || z >= g.gs[2]) return kVfeEmpty;
   *ix = x; *iy = y; *iz = z;
   return (unsigned)((z * g.gs[1] + y) * g.gs[0] + x);
@@ -182,7 +190,7 @@ struct lsd_vfe {
   lsd::VfeGrid grid{};
   int device = 0;
   cudaStream_t stream = nullptr;
-  float* pts[2] = {nullptr, nullptr};  // A/B sliding-window buffers (preprocess_kernel.cu:44-49)
+  float* pts[2] = {nullptr, nullptr};  // A/B sliding-window buffers (preprocess_kernel.cu:44-49), rows() rows each
   int cur = 0;
   std::vector<int> frame_pts;
   int total = 0;
@@ -196,6 +204,11 @@ struct lsd_vfe {
   unsigned* npts = nullptr;
   int num_voxels = 0;
   long long launches = 0;
+  // The window's row bound.  The reference's arithmetic (kept: the totals are its totals) gives an incoming frame at
+  // least one row even when the remaining frames already fill max_points, and a frame slot that was never filled pops 0
+  // rows, so the total can reach max_points + max_frame_num - 1 (e.g. frames of max_points rows: max_points,
+  // max_points + 1, ..., then back to max_points once a full frame leaves).
+  size_t rows() const { return (size_t)p.max_points + (size_t)p.max_frame_num - 1; }
 };
 
 using namespace lsd;
@@ -212,7 +225,14 @@ void lsd_vfe_default_params(lsd_vfe_params_t* p) {
 
 lsd_status_t lsd_vfe_create(lsd_vfe_t** out, const lsd_vfe_params_t* p) {
   if (!out || !p || p->num_feature < 4 || p->num_feature > 8 || p->max_points_per_voxel < 1 || p->max_points_per_voxel > 5 ||
-      p->max_points < 1 || p->max_voxels < 1 || p->max_frame_num < 1) { set_error("lsd_vfe_create: bad params"); return LSD_ERR_INVALID; }
+      p->max_points < 1 || p->max_voxels < 1 || p->max_frame_num < 1 || (long long)p->max_points + p->max_frame_num - 1 > INT_MAX) {
+    set_error("lsd_vfe_create: bad params"); return LSD_ERR_INVALID;
+  }
+  int gs[3];
+  for (int i = 0; i < 3; i++) gs[i] = (int)std::round((p->max_range[i] - p->min_range[i]) / p->voxel_size[i]);  // compute_grid_size, :182-189
+  if ((long long)gs[0] * gs[1] * gs[2] >= (1ll << 31)) {  // voxel keys (z * gs1 + y) * gs0 + x are 32-bit ints
+    set_error("lsd_vfe_create: grid of 2^31 cells or more"); return LSD_ERR_INVALID;
+  }
   lsd_status_t s = ensure_device();
   if (s) return s;
   lsd_vfe* v = new lsd_vfe();
@@ -220,20 +240,20 @@ lsd_status_t lsd_vfe_create(lsd_vfe_t** out, const lsd_vfe_params_t* p) {
   cudaGetDevice(&v->device);
   for (int i = 0; i < 3; i++) {
     v->grid.mn[i] = p->min_range[i]; v->grid.mx[i] = p->max_range[i]; v->grid.vs[i] = p->voxel_size[i];
-    v->grid.gs[i] = (int)std::round((p->max_range[i] - p->min_range[i]) / p->voxel_size[i]);  // compute_grid_size, :182-189
+    v->grid.gs[i] = gs[i];
   }
   v->grid.max_ppv = p->max_points_per_voxel; v->grid.max_voxels = p->max_voxels; v->grid.nf = p->num_feature;
   v->frame_pts.assign(p->max_frame_num, 0);
-  unsigned cap = 1024;
-  while (cap < (unsigned)p->max_points * 2u) cap <<= 1;
-  v->mask = cap - 1;
-  const size_t N = (size_t)p->max_points;
+  const size_t N = v->rows();
+  size_t cap = 1024;
+  while (cap < N * 2) cap <<= 1;
+  v->mask = (unsigned)(cap - 1);
   cudaError_t e = cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking);
   auto A = [&](void** ptr, size_t b) { if (e == cudaSuccess) e = cudaMalloc(ptr, b); if (e == cudaSuccess) e = cudaMemset(*ptr, 0, b); };
   A((void**)&v->pts[0], N * p->num_feature * 4);
   A((void**)&v->pts[1], N * p->num_feature * 4);
   A((void**)&v->d_motion, 64);
-  A((void**)&v->tab, (size_t)cap * sizeof(VfeSlot));
+  A((void**)&v->tab, cap * sizeof(VfeSlot));
   A((void**)&v->pslot, N * 4);
   A((void**)&v->local, N * 4);
   A((void**)&v->block_sum, (N / 1024 + 2) * 4);
@@ -243,8 +263,8 @@ lsd_status_t lsd_vfe_create(lsd_vfe_t** out, const lsd_vfe_params_t* p) {
   A((void**)&v->idx, (size_t)p->max_voxels * 16);
   A((void**)&v->npts, (size_t)p->max_voxels * 4);
   if (e == cudaSuccess) {  // idle state of a slot: key empty, count 0, sel = +inf
-    std::vector<unsigned> init((size_t)cap * 8);
-    for (size_t i = 0; i < (size_t)cap; i++) { unsigned* q = &init[i * 8]; q[0] = kVfeEmpty; q[1] = 0; for (int k = 2; k < 7; k++) q[k] = kVfeEmpty; q[7] = 0; }
+    std::vector<unsigned> init(cap * 8);
+    for (size_t i = 0; i < cap; i++) { unsigned* q = &init[i * 8]; q[0] = kVfeEmpty; q[1] = 0; for (int k = 2; k < 7; k++) q[k] = kVfeEmpty; q[7] = 0; }
     e = cudaMemcpy(v->tab, init.data(), init.size() * 4, cudaMemcpyHostToDevice);
   }
   if (e != cudaSuccess) { lsd_status_t r = cuda_fail(e, "lsd_vfe_create", __FILE__, __LINE__); lsd_vfe_destroy(v); return r; }
@@ -266,10 +286,14 @@ lsd_status_t lsd_vfe_destroy(lsd_vfe_t* v) {
 // PreprocessImplement::forward (preprocess_kernel.cu:56-101)
 lsd_status_t lsd_vfe_accumulate(lsd_vfe_t* v, const float* points_host, int num_points, const float* motion16_host, int realtime,
                                 int* total_points) {
-  if (!v || !points_host || num_points < 0 || (realtime && !motion16_host)) return LSD_ERR_INVALID;
+  if (!v || (!points_host && num_points > 0) || num_points < 0 || (realtime && !motion16_host)) return LSD_ERR_INVALID;
   LSD_CUDA(cudaSetDevice(v->device));
   cudaStream_t st = v->stream;
   const int nf = v->p.num_feature;
+  // the one row the reference counts for an empty realtime frame (and copies from the caller's empty array): far out,
+  // finite, outside every range box after any rigid motion
+  float far_row[8] = {1e30f, 1e30f, 1e30f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (realtime && num_points == 0) points_host = far_row;
   if (realtime) {
     LSD_CUDA(cudaMemcpyAsync(v->d_motion, motion16_host, 64, cudaMemcpyHostToDevice, st));
     v->total -= v->frame_pts.back();
@@ -292,7 +316,7 @@ lsd_status_t lsd_vfe_accumulate(lsd_vfe_t* v, const float* points_host, int num_
   }
   v->frame_pts[0] = num_points;
   v->total += num_points;
-  LSD_CUDA(cudaMemcpyAsync(v->pts[v->cur], points_host, (size_t)num_points * nf * 4, cudaMemcpyHostToDevice, st));
+  if (num_points > 0) LSD_CUDA(cudaMemcpyAsync(v->pts[v->cur], points_host, (size_t)num_points * nf * 4, cudaMemcpyHostToDevice, st));
   LSD_CUDA(cudaStreamSynchronize(st));
   if (total_points) *total_points = v->total;
   return LSD_OK;

@@ -7,10 +7,33 @@ executed SEQUENTIALLY in point order (the reference's GPU result depends on thre
 the sequential order is one of its possible outcomes).  Pin status: the reference has no CPU implementation of this
 path, but its two .cu files recompile unmodified for sm_90a (oracle/ref_vfe.cu -> oracle/_ref/libref_vfe.so, class
 RefVoxelizer below) and pin this restatement's semantics and the product on the GPU box (tests/test_gpu_ref_cuda.py).
+Where the product deviates from the reference on purpose (include/lsdreg.h), this follows the product: the row counted for
+an empty realtime frame is FAR_ROW_XYZ, and the window transform carries every feature past z (time + 0.1 only when
+num_feature > 4).
 """
 from __future__ import annotations
 
 import numpy as np
+
+# The row lsd_vfe_accumulate counts for an empty realtime frame (the reference counts one row there and copies it from
+# the caller's empty array): finite, and far enough out that no rigid motion brings it into a range box.
+FAR_ROW_XYZ = 1e30
+
+
+def fma32(a, b, c):
+    """fp32 fma(a, b, c), correctly rounded, on arrays.  a*b is exact in float64; TwoSum gives s + e == a*b + c exactly,
+    and s rounds to the fp32 nearest a*b + c unless s is itself halfway between two floats, where e breaks the tie."""
+    a64, b64, c64 = (np.asarray(v, np.float32).astype(np.float64) for v in (a, b, c))
+    with np.errstate(invalid="ignore", over="ignore"):
+        p = a64 * b64
+        s = p + c64
+        bb = s - p
+        e = (p - (s - bb)) + (c64 - bb)
+        r = s.astype(np.float32)
+        other = np.nextafter(r, np.where(s > r.astype(np.float64), np.float32(np.inf), np.float32(-np.inf)))
+        mid = s == (r.astype(np.float64) + other.astype(np.float64)) * 0.5
+        to_other = mid & np.isfinite(s) & (e != 0) & ~np.isnan(e) & ((e > 0) == (other > r))
+    return np.where(to_other, other, r).astype(np.float32)
 
 
 class OracleVoxelizer:
@@ -26,24 +49,28 @@ class OracleVoxelizer:
         self.buf = np.zeros((0, nf), np.float32)
 
     def accumulate(self, pts, motion=None, realtime=True):
-        pts = np.ascontiguousarray(pts, np.float32)
+        pts = np.ascontiguousarray(pts, np.float32).reshape(-1, self.nf)
         n = pts.shape[0]
         if realtime:
             m = np.ascontiguousarray(np.eye(4) if motion is None else motion, np.float32).ravel()
             self.total -= self.frame_pts[-1]
             n = max(min(n, self.max_points - self.total), 1)
+            if pts.shape[0] == 0:                                    # the one counted row of an empty frame
+                pts = np.zeros((1, self.nf), np.float32)
+                pts[0, :3] = FAR_ROW_XYZ
             self.frame_pts = [0] + self.frame_pts[:-1]
             old = self.buf[:self.total]
-            out = old.copy()
+            out = old.copy()                                         # features 3.. carried over
             if self.total > 0:
-                x, y, z = old[:, 0].astype(np.float64), old[:, 1].astype(np.float64), old[:, 2].astype(np.float64)
-                for r in range(3):  # as nvcc contracts the reference's m0*x + m1*y + m2*z + m3 (SASS of transform_kernel:
-                    # FMUL m1*y; FFMA m0*x + .; FFMA m2*z + .; FADD m3), each step rounded to fp32
-                    t = (np.float64(m[4 * r + 1]) * y).astype(np.float32)
-                    t = (np.float64(m[4 * r]) * x + t.astype(np.float64)).astype(np.float32)
-                    t = (np.float64(m[4 * r + 2]) * z + t.astype(np.float64)).astype(np.float32)
-                    out[:, r] = t + m[4 * r + 3]
-                out[:, 4] = (old[:, 4].astype(np.float64) + 0.1).astype(np.float32)
+                with np.errstate(invalid="ignore", over="ignore"):
+                    for r in range(3):  # as nvcc contracts the reference's m0*x + m1*y + m2*z + m3 (SASS of transform_kernel:
+                        # FMUL m1*y; FFMA m0*x + .; FFMA m2*z + .; FADD m3), each step rounded to fp32
+                        t = m[4 * r + 1] * old[:, 1]
+                        t = fma32(m[4 * r], old[:, 0], t)
+                        t = fma32(m[4 * r + 2], old[:, 2], t)
+                        out[:, r] = t + m[4 * r + 3]
+                    if self.nf > 4:                                  # the time channel
+                        out[:, 4] = (old[:, 4].astype(np.float64) + 0.1).astype(np.float32)
             self.buf = np.concatenate([pts[:n], out], 0)
         else:
             self.frame_pts = [0] * len(self.frame_pts)
@@ -54,16 +81,28 @@ class OracleVoxelizer:
         self.total += n
         return self.total
 
+    def cells(self, points):
+        """Per point: its cell (x, y, z) = floor((p - min) / voxel_size) in fp32, whether it passes the range test
+        (min <= p < max per axis) and whether its cell lies in the grid.  NaN on an axis passes the range test and
+        lands in cell 0 of that axis: the comparisons are false and the device's float-to-int conversion gives 0."""
+        p = np.ascontiguousarray(points, np.float32)
+        ijk = np.zeros((p.shape[0], 3), np.int64)
+        in_range = np.ones(p.shape[0], bool)
+        in_grid = np.ones(p.shape[0], bool)
+        for a in range(3):
+            c = p[:, a]
+            with np.errstate(invalid="ignore", over="ignore"):
+                q = np.floor((c - self.mn[a]) / self.vs[a])
+            q = np.where(np.isnan(q), 0.0, np.clip(q, -1.0, float(self.gs[a])))
+            ijk[:, a] = q.astype(np.int64)
+            in_range &= ((c >= self.mn[a]) & (c < self.mx[a])) | np.isnan(c)
+            in_grid &= (ijk[:, a] >= 0) & (ijk[:, a] < self.gs[a])
+        return ijk, in_range, in_grid
+
     def voxelize(self, points=None, zyx=True):
         p = self.buf[:self.total] if points is None else np.ascontiguousarray(points, np.float32)
-        n = p.shape[0]
-        inr = np.ones(n, bool)
-        ijk = np.zeros((n, 3), np.int64)
-        for a in range(3):
-            inr &= (p[:, a] >= self.mn[a]) & (p[:, a] < self.mx[a])
-            ijk[:, a] = np.floor((p[:, a] - self.mn[a]) / self.vs[a]).astype(np.int64)
-        for a in range(3):
-            inr &= (ijk[:, a] >= 0) & (ijk[:, a] < self.gs[a])
+        ijk, in_range, in_grid = self.cells(p)
+        inr = in_range & in_grid
         ids = np.nonzero(inr)[0]
         off = (ijk[ids, 2] * self.gs[1] + ijk[ids, 1]) * self.gs[0] + ijk[ids, 0]
         uniq, first, inv, cnt = np.unique(off, return_index=True, return_inverse=True, return_counts=True)
@@ -75,19 +114,20 @@ class OracleVoxelizer:
         start = np.searchsorted(gv, np.arange(len(uniq)))
         feat = np.zeros((V, self.nf), np.float32)
         npts = np.minimum(cnt[vorder][:V], self.max_ppv).astype(np.uint32)
-        for k in range(self.max_ppv):
-            has = npts > k
-            src = ids[srt[start[:V][has] + k]]
-            if k == 0:
-                feat[has] = p[src]
-            else:
-                feat[has] = feat[has] + p[src]                # fp32, sequential order
-        feat = feat / npts[:, None].astype(np.float32)
+        with np.errstate(invalid="ignore", over="ignore"):
+            for k in range(self.max_ppv):
+                has = npts > k
+                src = ids[srt[start[:V][has] + k]]
+                if k == 0:
+                    feat[has] = p[src]
+                else:
+                    feat[has] = feat[has] + p[src]            # fp32, sequential order
+            feat = (feat / npts[:, None].astype(np.float32)).astype(np.float16)
         firstpt = ids[first[vorder][:V]]
         idx = np.zeros((V, 4), np.uint32)
         c = ijk[firstpt]
         idx[:, 1:] = c[:, ::-1] if zyx else c
-        return feat.astype(np.float16), idx, npts
+        return feat, idx, npts
 
 
 class RefVoxelizer:

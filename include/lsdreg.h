@@ -386,7 +386,8 @@ lsd_status_t lsd_reg_align(lsd_reg_t* r, const float* guess16, float* out16, int
 lsd_status_t lsd_reg_iteration_log(lsd_reg_t* r, double* out4_per_iter, int cap_iters, int* n_iters);
 lsd_status_t lsd_reg_get_final(lsd_reg_t* r, double* T16, double* H36);           /* double pose, getFinalHessian */
 /* getFitnessScore(max_range) at T16 (NULL = the final transformation).  NB PCL compares the SQUARED
- * nearest-neighbour distance with max_range. */
+ * nearest-neighbour distance with max_range.  The nearest neighbour is exact at any range: past the point map's grid
+ * search (64 map voxels) and on a target whose point map refused points, it comes from a scan of the whole target. */
 lsd_status_t lsd_reg_fitness(lsd_reg_t* r, const double* T16_or_null, double max_range, double* score);
 /* One cost evaluation (parity tap): update != 0 = linearize(T) (correspondences refreshed), else
  * compute_error(T).  H36/b6 may be NULL. */

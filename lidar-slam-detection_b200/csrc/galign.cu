@@ -21,6 +21,7 @@ namespace lsd {
 struct GaCand {
   VgView vg;             // cost: the reference key frame's VGICP voxel table
   MapView mv;            // fitness: the reference key frame's point map
+  NnTarget tg;           // fitness: its cloud as the fallback of the map's grid search (fitness_target)
   Pose34d T;             // cost: evaluation pose (linearisation pose when update)
   Pose34f Tf;            // fitness: the pose, in float as getFitnessScore applies it
   long long corr_off;    // cost: [n_off, n] correspondence slots and 6 [n_off, n] Mahalanobis doubles at this offset of the pools
@@ -69,9 +70,9 @@ __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_pairs_kernel(const 
   const Pose34f Tf = cands[c].Tf;
   const float4* src = pool + cands[c].src_off;
   if (cands[c].warp_shape)  // block-uniform
-    fitness_range<true>(mv, src, n, lb, G, Tf, search_sq, max_range, nullptr, 0, partials);
+    fitness_range<true>(mv, src, n, lb, G, Tf, search_sq, max_range, cands[c].tg, partials);
   else
-    fitness_range<false>(mv, src, n, lb, G, Tf, search_sq, max_range, nullptr, 0, partials);
+    fitness_range<false>(mv, src, n, lb, G, Tf, search_sq, max_range, cands[c].tg, partials);
   loop_finalize<2>(partials + (size_t)cands[c].blk_off * kNV, G, done + 1 + c, done, n_cand,
                    result + (size_t)(1 + cands[c].row) * kNV, result, seq);
 }
@@ -191,7 +192,9 @@ static lsd_status_t ga_fitness(lsd_galign* h, const std::vector<GaPair>& pairs, 
   for (int i = 0; i < n; i++) {
     GaCand& c = h->b.h_cand[i];
     memset(&c, 0, sizeof(c));
-    c.mv = h->tgt[pairs[i].ref_slot].map->view;
+    const int ref = pairs[i].ref_slot;
+    c.mv = h->tgt[ref].map->view;
+    c.tg = fitness_target(h->tgt[ref].map, h->d_pool + h->kf_off[ref], h->kf_n[ref], h->p.fitness_score_max_range, h->p.reg.map_resolution);
     c.src_off = (int)h->kf_off[pairs[i].new_slot]; c.n = h->kf_n[pairs[i].new_slot]; c.row = i;
     c.warp_shape = c.n < kThreadShapeMin;
     c.n_blk = c.warp_shape ? warp_grid(c.n) : reg_grid(c.n);

@@ -106,10 +106,10 @@ __global__ void __launch_bounds__(256) ndt_cost_batch_kernel(NdtView v, const fl
 
 // getFitnessScore(max_range) of every candidate at its pose against the new key frame's point map.  Per candidate the
 // shape and grid of lsd_reg_fitness and the same body (fitness_range, reg.cu) and fold: same sum, same count.
-// tgt != nullptr: points with no neighbour within search_sq get the exact one, for calc_fitness_score.
+// tg: the new key frame's cloud as the fallback of the map's grid search (fitness_target).
 __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_batch_kernel(MapView mv, const float4* __restrict__ pool,
                                                                           const LoopCand* __restrict__ cands, int n_cand, float search_sq,
-                                                                          double max_range, const float4* __restrict__ tgt, int n_tgt,
+                                                                          double max_range, NnTarget tg,
                                                                           double* __restrict__ partials, unsigned* __restrict__ done,
                                                                           double* __restrict__ result, double seq) {
   const int c = loop_cand_of_block(cands, n_cand);
@@ -117,9 +117,9 @@ __global__ void __launch_bounds__(kRegWarps * 32, 2) fitness_batch_kernel(MapVie
   const Pose34f Tf = cands[c].ev;
   const float4* src = pool + cands[c].src_off;
   if (cands[c].warp_shape)  // block-uniform
-    fitness_range<true>(mv, src, n, lb, G, Tf, search_sq, max_range, tgt, n_tgt, partials);
+    fitness_range<true>(mv, src, n, lb, G, Tf, search_sq, max_range, tg, partials);
   else
-    fitness_range<false>(mv, src, n, lb, G, Tf, search_sq, max_range, tgt, n_tgt, partials);
+    fitness_range<false>(mv, src, n, lb, G, Tf, search_sq, max_range, tg, partials);
   loop_finalize<2>(partials + (size_t)cands[c].blk_off * kNV, G, done + 1 + c, done, n_cand,
                    result + (size_t)(1 + cands[c].row) * kNV, result, seq);
 }
@@ -237,7 +237,7 @@ static lsd_status_t loop_set_target(lsd_loop* h, int slot, long long* launches) 
 
 // One fitness launch for candidates (slot, pose) against the current target; score[i] as getFitnessScore returns it.
 static lsd_status_t loop_fitness(lsd_loop* h, const std::vector<int>& slots, const std::vector<Pose34f>& poses, double max_range,
-                                 bool exact, double* score, double* count, long long* launches) {
+                                 double* score, double* count, long long* launches) {
   const int n = (int)slots.size();
   if (n == 0) return LSD_OK;
   lsd_reg* r = h->ndt;
@@ -261,7 +261,8 @@ static lsd_status_t loop_fitness(lsd_loop* h, const std::vector<int>& slots, con
   if (s) return s;
   const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
   fitness_batch_kernel<<<blocks, kRegWarps * 32, 0, st>>>(r->tgt_map->view, h->d_pool, h->b.d_cand, n, search_sq, max_range,
-                                                         exact ? r->d_tgt : nullptr, r->n_tgt, h->b.d_partials, h->b.d_done, h->b.d_res, seq);
+                                                         fitness_target(r->tgt_map, r->d_tgt, r->n_tgt, max_range, r->p.map_resolution),
+                                                         h->b.d_partials, h->b.d_done, h->b.d_res, seq);
   LSD_CUDA(cudaGetLastError());
   (*launches)++;
   s = h->b.wait(st, seq);
@@ -329,7 +330,7 @@ static lsd_status_t loop_coarse(lsd_loop* h, int target, const int32_t* cand, co
   std::vector<Pose34f> poses(n);
   for (int i = 0; i < n; i++) T_to_pose(h->lm[i].x0, nullptr, &poses[i]);
   h->fitness.assign(n, 0.0);
-  return loop_fitness(h, slots, poses, h->p.fitness_score_max_range, false, h->fitness.data(), nullptr, launches);
+  return loop_fitness(h, slots, poses, h->p.fitness_score_max_range, h->fitness.data(), nullptr, launches);
 }
 
 // Eigen::Quaterniond(R).normalized().toRotationMatrix() (Eigen/src/Geometry/Quaternion.h quaternionbase_assign_impl,
@@ -546,7 +547,7 @@ lsd_status_t lsd_loop_fitness(lsd_loop_t* h, int32_t target_slot, int32_t source
   std::vector<Pose34f> pose(1);
   T_to_pose(T, nullptr, &pose[0]);
   double cnt = 0;
-  s = loop_fitness(h, std::vector<int>{source_slot}, pose, max_range, true, score, &cnt, &ln);
+  s = loop_fitness(h, std::vector<int>{source_slot}, pose, max_range, score, &cnt, &ln);
   if (n_counted) *n_counted = (int)(cnt + 0.5);
   return s;
 }

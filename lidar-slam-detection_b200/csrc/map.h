@@ -39,6 +39,7 @@ struct lsd_map {
   size_t bscratch_bytes = 0;
   LruMirror* lru = nullptr;        // lsd_map_enable_lru
   unsigned long long dropped_seen = 0;   // counters[2] at the last look (lsd_map_saturated)
+  bool incomplete = false;   // a matcher's point map (build_point_map, reg.cu) refused points: its grid search is not exact
 };
 
 namespace lsd {

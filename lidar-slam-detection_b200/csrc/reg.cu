@@ -372,6 +372,41 @@ __device__ __forceinline__ bool nn1_exact_thread(const MapView& mv, float qx, fl
   return found;
 }
 
+// The cloud behind a target point map (its ids are the indices 0 .. n - 1), for the searches the map cannot serve exactly.
+// all != 0: the map refused points (lsd_map::incomplete, build_point_map), so every search scans pts instead of the map;
+// else pts, when not null, serves only the points with nothing within the grid search radius (fitness_target).
+struct NnTarget { const float4* pts; int n; int all; };
+
+// Exact nearest neighbour (d2, target index) by a scan of the whole target, ties to the lower index as in the grid search
+// (index -1 and 3e38 when nothing was scanned).  Thread version: ascending j, so a strict < keeps the lower index.
+__device__ __forceinline__ float nn_scan_thread(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz, int* id) {
+  float bd = 3.0e38f; int bi = -1;
+  for (int j = 0; j < n_tgt; j++) {
+    const float4 b = __ldg(tgt + j);
+    const float d2 = dist2(qx, qy, qz, b.x, b.y, b.z);
+    if (d2 < bd) { bd = d2; bi = j; }
+  }
+  *id = bi;
+  return bd;
+}
+// Warp version: lanes stride over the target, then the (d2, index) minimum across lanes (every lane returns it).
+__device__ __forceinline__ float nn_scan_warp(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz, int* id) {
+  float bd = 3.0e38f; int bi = -1;
+  for (int j = threadIdx.x & 31; j < n_tgt; j += 32) {
+    const float4 b = __ldg(tgt + j);
+    const float d2 = dist2(qx, qy, qz, b.x, b.y, b.z);
+    if (d2 < bd) { bd = d2; bi = j; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float od = __shfl_xor_sync(0xffffffffu, bd, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (od < bd || (od == bd && (unsigned)oi < (unsigned)bi)) { bd = od; bi = oi; }   // -1 (nothing scanned) sorts last
+  }
+  *id = bi;
+  return bd;
+}
+
 // Mahalanobis matrix (C_B + R C_A R^T)^-1 of correspondence (source i, target c) at T, in double, stored symmetric
 // (xx xy xz yy yz zz) into maha[6 i ..].
 __device__ __forceinline__ void gicp_store_maha(const double* __restrict__ src_nrm, const double* __restrict__ tgt_nrm, int i, int c,
@@ -395,8 +430,9 @@ __device__ __forceinline__ void gicp_store_maha(const double* __restrict__ src_n
 // update_correspondences (fast_gicp_impl.hpp:119-157): 1-NN of the transformed source point, Mahalanobis
 // matrix.  One warp per source point.  The reference keeps the neighbour when its FLOAT squared distance is below the DOUBLE
 // max_corr_dist^2 (fast_gicp_impl.hpp:141): gate with max_corr_sq in double; search_sq (corr_search_sq) is the inclusive
-// float bound of the grid search that holds every float below it.
-__global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv, const float4* __restrict__ src,
+// float bound of the grid search that holds every float below it.  tg.all (an incomplete target map): the 1-NN by a scan of
+// the whole target instead, the same (d2, index) minimum the grid search of a complete map finds.
+__global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv, NnTarget tg, const float4* __restrict__ src,
                                                                       const double* __restrict__ src_nrm, int n,
                                                                       const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
                                                                       float search_sq, double max_corr_sq, int* __restrict__ corr,
@@ -406,27 +442,35 @@ __global__ void __launch_bounds__(kRegWarps * 32, 3) gicp_corr_kernel(MapView mv
   WarpList wl = make_warp_list(s_list, warp);
   for (int i = blockIdx.x * kRegWarps + warp; i < n; i += gridDim.x * kRegWarps) {
     const float3 q = xform(Tf, __ldg(src + i));
-    Neighbor nb;
-    const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, search_sq, wl, nb);
-    const float d2 = __shfl_sync(kFull, nb.d2, 0);
-    const int id = __shfl_sync(kFull, nb.id, 0);
+    float d2; int id;
+    if (tg.all) {                                                      // grid-uniform
+      d2 = nn_scan_warp(tg.pts, tg.n, q.x, q.y, q.z, &id);
+    } else {
+      Neighbor nb;
+      const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, search_sq, wl, nb);
+      d2 = __shfl_sync(kFull, nb.d2, 0);
+      const int nid = __shfl_sync(kFull, nb.id, 0);
+      id = nf > 0 ? nid : -1;
+    }
     if (lane != 0) continue;
-    const int c = (nf > 0 && (double)d2 < max_corr_sq) ? id : -1;
+    const int c = (id >= 0 && (double)d2 < max_corr_sq) ? id : -1;
     corr[i] = c;
     if (c >= 0) gicp_store_maha(src_nrm, tgt_nrm, i, c, T, maha);
   }
 }
 
-// update_correspondences, batched shape: one thread per source point (nn1_exact_thread)
-__global__ void __launch_bounds__(256) gicp_corr_thread_kernel(MapView mv, const float4* __restrict__ src, const double* __restrict__ src_nrm,
-                                                               int n, const double* __restrict__ tgt_nrm, Pose34d T, Pose34f Tf,
-                                                               float search_sq, double max_corr_sq, int* __restrict__ corr,
-                                                               double* __restrict__ maha) {
+// update_correspondences, batched shape: one thread per source point (nn1_exact_thread; tg.all: nn_scan_thread)
+__global__ void __launch_bounds__(256) gicp_corr_thread_kernel(MapView mv, NnTarget tg, const float4* __restrict__ src,
+                                                               const double* __restrict__ src_nrm, int n, const double* __restrict__ tgt_nrm,
+                                                               Pose34d T, Pose34f Tf, float search_sq, double max_corr_sq,
+                                                               int* __restrict__ corr, double* __restrict__ maha) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float3 q = xform(Tf, __ldg(src + i));
   float d2; int id;
-  const bool f = nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
+  bool f;
+  if (tg.all) { d2 = nn_scan_thread(tg.pts, tg.n, q.x, q.y, q.z, &id); f = id >= 0; }
+  else f = nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
   const int c = (f && (double)d2 < max_corr_sq) ? id : -1;
   corr[i] = c;
   if (c >= 0) gicp_store_maha(src_nrm, tgt_nrm, i, c, T, maha);
@@ -620,32 +664,16 @@ __global__ void __launch_bounds__(256) vgicp_cost_kernel(VgView v, const float4*
   grid_finalize<29>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
 
-// Exact nearest-neighbour distance by a scan of the whole target, for points with nothing inside the grid search radius:
-// calc_fitness_score counts every point however far (max_range = DBL_MAX).  Thread version.
-__device__ __forceinline__ float nn_scan_thread(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz) {
-  float bd = 3.0e38f;
-  for (int j = 0; j < n_tgt; j++) { const float4 b = __ldg(tgt + j); bd = fminf(bd, dist2(qx, qy, qz, b.x, b.y, b.z)); }
-  return bd;
-}
-// Warp version: lanes stride over the target, then a min across lanes (every lane returns it).
-__device__ __forceinline__ float nn_scan_warp(const float4* __restrict__ tgt, int n_tgt, float qx, float qy, float qz) {
-  float bd = 3.0e38f;
-  for (int j = threadIdx.x & 31; j < n_tgt; j += 32) { const float4 b = __ldg(tgt + j); bd = fminf(bd, dist2(qx, qy, qz, b.x, b.y, b.z)); }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) bd = fminf(bd, __shfl_xor_sync(0xffffffffu, bd, o));
-  return bd;
-}
-
 // getFitnessScore (sum of squared 1-NN distances <= max_range, and their count) over block lb of the G blocks a cloud of n
 // points gets, stored as the block's row (sum, count) of partials.  As in the reference, the float d2 is compared with the
 // double max_range (PCL's `nn_dists[0] <= max_range`).  WARP: one warp per point (knn_exact_warp), else one
-// thread per point (nn1_exact_thread).  tgt != nullptr: points with no neighbour within search_sq get the exact one by a
-// scan of the whole target (nn_scan_*), for calc_fitness_score.  The single-pair kernel and the loop detector's batched
-// kernel (loop.cu) both run this body, so a candidate's row has the single-pair bits.
+// thread per point (nn1_exact_thread).  tg (fitness_target): with tg.all every point gets its nearest neighbour by a scan
+// of the whole target (nn_scan_*), the map being incomplete; else, with tg.pts, the points with no neighbour within
+// search_sq do, max_range reaching past the grid search.  The single-pair kernel and the batched kernels of the loop
+// detector (loop.cu) and the global aligner (galign.cu) all run this body, so a candidate's row has the single-pair bits.
 template <bool WARP>
 __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* __restrict__ src, int n, int lb, int G, const Pose34f& Tf,
-                                              float search_sq, double max_range, const float4* __restrict__ tgt, int n_tgt,
-                                              double* __restrict__ partials) {
+                                              float search_sq, double max_range, const NnTarget& tg, double* __restrict__ partials) {
   __shared__ double s_acc[kRegWarps][2];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   double sum = 0.0, cnt = 0.0;
@@ -654,19 +682,22 @@ __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* _
     WarpList wl = make_warp_list(s_list, warp);
     for (int i = lb * kRegWarps + warp; i < n; i += G * kRegWarps) {
       const float3 q = xform(Tf, __ldg(src + i));
-      Neighbor nb;
-      const int nf = knn_exact_warp<1>(mv, q.x, q.y, q.z, search_sq, wl, nb);
-      float d2 = __shfl_sync(kFull, nb.d2, 0);
-      bool found = nf > 0;
-      if (!found && tgt) { d2 = nn_scan_warp(tgt, n_tgt, q.x, q.y, q.z); found = n_tgt > 0; }   // warp-uniform
+      float d2 = 3.0e38f; int id;
+      bool found = false;
+      if (!tg.all) {                                                   // block-uniform
+        Neighbor nb;
+        found = knn_exact_warp<1>(mv, q.x, q.y, q.z, search_sq, wl, nb) > 0;
+        d2 = __shfl_sync(kFull, nb.d2, 0);
+      }
+      if (!found && tg.pts) { d2 = nn_scan_warp(tg.pts, tg.n, q.x, q.y, q.z, &id); found = tg.n > 0; }   // warp-uniform
       if (found && (double)d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
     }
   } else {
     for (int i = lb * blockDim.x + threadIdx.x; i < n; i += G * blockDim.x) {
       const float3 q = xform(Tf, __ldg(src + i));
-      float d2; int id;
-      bool found = nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
-      if (!found && tgt) { d2 = nn_scan_thread(tgt, n_tgt, q.x, q.y, q.z); found = n_tgt > 0; }
+      float d2 = 3.0e38f; int id;
+      bool found = !tg.all && nn1_exact_thread(mv, q.x, q.y, q.z, search_sq, &d2, &id);
+      if (!found && tg.pts) { d2 = nn_scan_thread(tg.pts, tg.n, q.x, q.y, q.z, &id); found = tg.n > 0; }
       if (found && (double)d2 <= max_range) { sum += (double)d2; cnt += 1.0; }
     }
     sum = warp_sum(sum); cnt = warp_sum(cnt);
@@ -684,10 +715,10 @@ __device__ __forceinline__ void fitness_range(const MapView& mv, const float4* _
 // shape asks for 3 blocks per SM, the thread shape for no minimum (0).
 template <bool WARP>
 __global__ void __launch_bounds__(kRegWarps * 32, WARP ? 3 : 0) fitness_kernel(MapView mv, const float4* __restrict__ src, int n,
-                                                                               Pose34f Tf, float search_sq, double max_range,
+                                                                               Pose34f Tf, float search_sq, double max_range, NnTarget tg,
                                                                                double* __restrict__ partials, unsigned* __restrict__ done,
                                                                                double* __restrict__ result, double seq, ShardComm sc) {
-  fitness_range<WARP>(mv, src, n, (int)blockIdx.x, (int)gridDim.x, Tf, search_sq, max_range, nullptr, 0, partials);
+  fitness_range<WARP>(mv, src, n, (int)blockIdx.x, (int)gridDim.x, Tf, search_sq, max_range, tg, partials);
   grid_finalize<2>(partials, done, result, 0, -1, 0.0, kResSeq, seq, sc, 0);
 }
 
@@ -747,8 +778,18 @@ static int warp_grid(int n) { return std::max(1, std::min((n + kRegWarps - 1) / 
 
 // getFitnessScore's grid search radius: max_range, at most 64 map voxels.  Rounded to the nearest float, the bound holds every
 // float <= max_range (the nearest float is either the largest float <= max_range or above it).
+static double fitness_search_cap(double map_resolution) { return 64.0 * map_resolution * map_resolution * 64.0; }
 static float fitness_search_sq(double max_range, double map_resolution) {
-  return (float)std::min(max_range, 64.0 * map_resolution * map_resolution * 64.0);
+  return (float)std::min(max_range, fitness_search_cap(map_resolution));
+}
+
+// The target cloud pts [n] behind the point map m as fitness_range's fallback: every point scans it when the map is
+// incomplete; else the points with nothing within the grid search radius do when max_range reaches past the cap (PCL
+// counts a neighbour however far), and nothing needs it otherwise.
+static NnTarget fitness_target(const lsd_map* m, const float4* pts, int n, double max_range, double map_resolution) {
+  if (m->incomplete) return NnTarget{pts, n, 1};
+  if (max_range > fitness_search_cap(map_resolution)) return NnTarget{pts, n, 0};
+  return NnTarget{nullptr, 0, 0};
 }
 
 // The inclusive float bound of update_correspondences' grid search for the gate (double)d2 < max_corr_sq: max_corr_sq
@@ -816,12 +857,13 @@ static lsd_status_t reg_cost(lsd_reg* r, const double* T, bool update, double* H
     if (update) {
       const double mc2 = r->p.max_corr_dist * r->p.max_corr_dist;
       const float search = corr_search_sq(mc2);
+      const NnTarget tg{r->d_tgt, r->n_tgt, r->tgt_map->incomplete ? 1 : 0};   // incomplete: scan the whole target
       if (r->n_src >= kThreadShapeMin)
-        gicp_corr_thread_kernel<<<(r->n_src + 255) / 256, 256, 0, st>>>(r->tgt_map->view, r->d_src, r->d_src_nrm, r->n_src, r->d_tgt_nrm, Td, Tf,
-                                                                        search, mc2, r->d_corr, r->d_maha);
+        gicp_corr_thread_kernel<<<(r->n_src + 255) / 256, 256, 0, st>>>(r->tgt_map->view, tg, r->d_src, r->d_src_nrm, r->n_src, r->d_tgt_nrm,
+                                                                        Td, Tf, search, mc2, r->d_corr, r->d_maha);
       else
-        gicp_corr_kernel<<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->d_src_nrm, r->n_src, r->d_tgt_nrm, Td, Tf,
-                                                                       search, mc2, r->d_corr, r->d_maha);
+        gicp_corr_kernel<<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, tg, r->d_src, r->d_src_nrm, r->n_src, r->d_tgt_nrm,
+                                                                       Td, Tf, search, mc2, r->d_corr, r->d_maha);
       r->launches++;
     }
     const int g = reg_grid(r->n_src);
@@ -1243,6 +1285,12 @@ lsd_status_t lsd_reg_shard_connect(lsd_reg_t* r, const unsigned char* blobs) {
   return LSD_OK;
 }
 
+// The exact-NN point map of the cloud d_pts [n] (ids 0 .. n - 1) into *mp, on the handle's stream, and (*mp)->incomplete:
+// whether the map refused any point.  It refuses a point of a voxel that already holds (kMaxLevel + 1) * kPtsPerLine
+// points (which a scan has where the sensor stands next to a wall), of a full probe chain, or beyond +-2^18 voxels, and
+// WHICH points of an overfull voxel it refuses depends on the order of the insert's atomics.  A grid search of an
+// incomplete map is then not exact, so every search of it scans the whole cloud instead: gicp_covariances here, the
+// correspondence kernels (reg_cost) and fitness_range (fitness_target).
 static lsd_status_t build_point_map(lsd_reg* r, lsd_map** mp, const float4* d_pts, int n) {
   const int l2 = r->p.map_log2_lines > 0 ? r->p.map_log2_lines : auto_log2((size_t)n, 12, 26);
   if (*mp && (*mp)->n_lines == (1ull << l2)) {
@@ -1261,7 +1309,12 @@ static lsd_status_t build_point_map(lsd_reg* r, lsd_map** mp, const float4* d_pt
   }
   lsd_status_t s = launch_insert(*mp, d_pts, n, 0, r->stream);
   (*mp)->stream = nullptr;
-  return s;
+  if (s) return s;
+  unsigned long long dropped = 0;
+  LSD_CUDA(cudaMemcpyAsync(&dropped, &(*mp)->view.counters[2], sizeof(dropped), cudaMemcpyDeviceToHost, r->stream));
+  LSD_CUDA(cudaStreamSynchronize(r->stream));
+  (*mp)->incomplete = dropped != 0;
+  return LSD_OK;
 }
 
 static void detach_map_stream(lsd_map* m) { if (m) m->stream = nullptr; }
@@ -1273,14 +1326,9 @@ static lsd_status_t gicp_covariances(lsd_reg* r, lsd_map** mp, const float4* d_p
   lsd_status_t s = build_point_map(r, mp, d_pts, n);
   if (s) return s;
   cudaStream_t st = r->stream;
-  // A point the map could not hold — a voxel of more than (kMaxLevel + 1) * kPtsPerLine points, which a scan has where the
-  // sensor stands next to a wall — is missing from the grid search, and WHICH points of such a voxel are missing depends on
-  // the order of the insert's atomics.  Then the grid search is not exact: every point takes the exact scan of the whole
-  // cloud instead (count column cleared, so gicp_normals_complete_kernel serves all of them).
-  unsigned long long dropped = 0;
-  LSD_CUDA(cudaMemcpyAsync(&dropped, &(*mp)->view.counters[2], sizeof(dropped), cudaMemcpyDeviceToHost, st));
-  LSD_CUDA(cudaStreamSynchronize(st));
-  if (dropped == 0) {
+  // An incomplete map (build_point_map): every point takes the exact scan of the whole cloud instead (count column
+  // cleared, so gicp_normals_complete_kernel serves all of them).
+  if (!(*mp)->incomplete) {
     gicp_normals_kernel<<<warp_grid(n), kRegWarps * 32, 0, st>>>((*mp)->view, d_pts, n, r->p.k_correspondences, (float)r->p.normal_search_sq, nrm);
     r->launches++;
   } else {
@@ -1440,11 +1488,12 @@ lsd_status_t lsd_reg_fitness(lsd_reg_t* r, const double* T16_or_null, double max
   T_to_pose(T16_or_null ? T16_or_null : r->final_T, nullptr, &Tf);
   const double seq = (double)(++r->seq);
   const float search_sq = fitness_search_sq(max_range, r->p.map_resolution);
+  const NnTarget tg = fitness_target(r->tgt_map, r->d_tgt, r->n_tgt, max_range, r->p.map_resolution);
   if (r->n_src >= kThreadShapeMin)
-    fitness_kernel<false><<<reg_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, max_range,
+    fitness_kernel<false><<<reg_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, max_range, tg,
                                                                          r->d_partials, r->d_done, r->d_result, seq, r->sc);
   else
-    fitness_kernel<true><<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, max_range,
+    fitness_kernel<true><<<warp_grid(r->n_src), kRegWarps * 32, 0, st>>>(r->tgt_map->view, r->d_src, r->n_src, Tf, search_sq, max_range, tg,
                                                                         r->d_partials, r->d_done, r->d_result, seq, r->sc);
   LSD_CUDA(cudaGetLastError());
   r->launches++;

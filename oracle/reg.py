@@ -182,12 +182,35 @@ class OracleMatcher:
         return x0
 
     def fitness(self, T=None, max_range=25.0):
+        """getFitnessScore(max_range): the mean fp32 squared distance from each source point (transformed in fp32) to its
+        nearest target point, over the points where it is <= max_range, however far that neighbour is.  Ranges up to 64
+        map voxels go through the grid search of orc_fitness, longer ones through a scan of the whole target."""
+        T = np.ascontiguousarray(self.final if T is None else T, np.float64)
+        if max_range > 64.0 * self.map_res * self.map_res * 64.0:
+            return _fitness_scan(self.tgt, self.src, T, max_range)
         if self.tmap is None:
             self.tmap = O.OracleIvox(self.map_res, 18, max(self.tgt.shape[0], 1024))
             self.tmap.add(np.ascontiguousarray(self.tgt[:, :3]), 0)
-        T = np.ascontiguousarray(self.final if T is None else T, np.float64)
-        return O.port.orc_fitness(self.tmap.h, self.src, self.src.shape[1], self.src.shape[0], T, max_range,
-                                  min(max_range, 64.0 * self.map_res * self.map_res * 64.0))
+        return O.port.orc_fitness(self.tmap.h, self.src, self.src.shape[1], self.src.shape[0], T, max_range, max_range)
+
+
+def _fitness_scan(tgt, src, T, max_range, chunk=256):
+    """orc_fitness by a scan of the whole target: the same fp32 transform ((r0 x + r1 y) + r2 z) + t and fp32 squared
+    distance (dx dx + dy dy) + dz dz, the float d2 compared with the double max_range, the sum in double in source order."""
+    R, t = T[:3, :3].astype(np.float32), T[:3, 3].astype(np.float32)
+    a = np.ascontiguousarray(src[:, :3], np.float32)
+    q = np.stack([R[r, 0] * a[:, 0] + R[r, 1] * a[:, 1] + R[r, 2] * a[:, 2] + t[r] for r in range(3)], 1)
+    P = np.ascontiguousarray(tgt[:, :3], np.float32)
+    best = np.empty(len(q), np.float32)
+    for i in range(0, len(q), chunk):
+        d = P[None, :, :] - q[i:i + chunk, None, :]
+        best[i:i + chunk] = (d[..., 0] * d[..., 0] + d[..., 1] * d[..., 1] + d[..., 2] * d[..., 2]).min(1)
+    s, nr = 0.0, 0
+    for v in best.astype(np.float64):
+        if v <= max_range:
+            s += v
+            nr += 1
+    return s / nr if nr > 0 else 1.7976931348623157e308
 
 
 class RefMatcher:

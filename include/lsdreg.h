@@ -577,6 +577,113 @@ lsd_status_t lsd_galign_cost(lsd_galign_t* h, int32_t new_slot, int32_t ref_slot
                              double* b6, double* err, int* n_corr);
 
 /* ------------------------------------------------------------------------------------------
+ * Overlap detector of map merging — replaces OverlapDetector::detect
+ * (slam/localization/include/overlap_merge.hpp:38-304, called from MapLoader::mergeMapSLAM,
+ * slam/localization/src/map_loader.cpp:118-137, when both maps share a GNSS origin).  Key-frame clouds (sensor frame) of
+ * both maps are uploaded once into one device pool, addressed by slot, with their graph id (KeyFrame::mId).  A key
+ * frame's NDT table, point map, filtered copy and that copy's point map are built on its first use as a target within a
+ * call; lsd_overlap_detect releases them when it returns (their buffers are reused by the next call), so device memory
+ * grows with the new key frames of one fragment, not with the size of the merge.
+ * lsd_overlap_detect does, for all new key frames of a fragment: find_candidates on the host (:113-145), the inlier
+ * prescreen of every (new, candidate) pair in one launch (:160-163), NDT_CUDA of every pair that passed with the
+ * Levenberg-Marquardt loops of all pairs advanced together (one batched cost launch per round, each pair bit-identical
+ * to lsd_reg's single-pair kernels on the same NDT table), getFitnessScore(25) of the converged pairs in one launch (:171), the best candidate
+ * per new key frame (:172-183), then per new key frame with a best candidate the accumulated target, FAST_GICP and the
+ * filtered fitness gate (:185-210).  graph_add_edge / graph_optimize / graph_sync_pose stay with the caller.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct lsd_overlap lsd_overlap_t;
+typedef struct lsd_overlap_params {
+  double distance_thresh;             /* 30.0 m between the key frames' translations (overlap_merge.hpp:46,132)          */
+  int32_t candidate_link_dist;        /* 10: a candidate needs get_connection_count(..., 10) >= 10 (:47,133-134)        */
+  int32_t max_candidate_num;          /* 3 candidates at most (:48,138)                                                 */
+  double fitness_score_max_range;     /* 25.0, SQUARED distance as PCL compares it (:49,171,204)                        */
+  double fitness_score_thresh;        /* 1.5: the finetune's filtered score must not exceed it (:50,205)                */
+  double fitness_inlier_thresh;       /* 0.2: the prescreen's inlier ratio must reach it (:51,161)                      */
+  double inlier_max_range;            /* 1.0, the prescreen's max_range (squared, :160)                                 */
+  double filter_range;                /* 100.0: filter() keeps sqrtf(x*x + y*y) < this, in float (:226)                 */
+  float filter_min_z;                 /* 0.5: and z > this (:227)                                                       */
+  lsd_reg_params_t coarse;            /* lsd_reg_default_params(LSD_REG_NDT_P2D): "NDT_CUDA" (:54), no timeout          */
+  lsd_reg_params_t accurate;          /* LSD_REG_GICP with max_corr_dist = 0.5, transformation_epsilon = 0.001 (:58-60)  */
+} lsd_overlap_params_t;
+
+typedef struct lsd_overlap_result {
+  int32_t key1, key2;          /* Overlap(key1 = best candidate slot, key2 = new key frame slot) (:210)               */
+  double relpose16[16];        /* registration_accurate->getFinalTransformation() (float) widened, row-major: new key
+                                  frame -> best candidate                                                             */
+  double score;                /* calc_fitness_score(accum, new, relpose, 25).first (:204)                             */
+  double coarse_score;         /* the best candidate's NDT getFitnessScore(25) (:171)                                  */
+} lsd_overlap_result_t;
+
+/* What detect decided for each new key frame (no reference counterpart beyond its LOG_INFO lines). */
+#define LSD_OVERLAP_NO_CANDIDATES 0   /* find_candidates returned nothing (:148-150)                                     */
+#define LSD_OVERLAP_NO_MATCH 1        /* every candidate failed the prescreen or did not converge (:181-183)             */
+#define LSD_OVERLAP_GICP_DIVERGED 2   /* the finetune did not converge (:200-202)                                        */
+#define LSD_OVERLAP_GICP_REJECT 3     /* the finetune's filtered score is above fitness_score_thresh (:205-207)          */
+#define LSD_OVERLAP_FOUND 4
+typedef struct lsd_overlap_report {
+  int32_t new_slot, decision;
+  int32_t n_candidates, n_prescreened;   /* candidates found / those whose inlier ratio reached fitness_inlier_thresh   */
+  int32_t best_slot;                     /* the coarse stage's choice, -1 = none                                         */
+  int32_t n_accum;                       /* points of the accumulated finetune target (0 when there was no best)         */
+  int32_t accum_incomplete;              /* the filtered accumulated target's point map refused points (searches scan it) */
+  double best_score;                     /* its NDT score (DBL_MAX when none)                                            */
+  double score;                          /* the finetune's filtered score (GICP_REJECT, FOUND), else 0                   */
+} lsd_overlap_report_t;
+
+void lsd_overlap_default_params(lsd_overlap_params_t* p);
+lsd_status_t lsd_overlap_create(lsd_overlap_t** out, const lsd_overlap_params_t* p);
+lsd_status_t lsd_overlap_destroy(lsd_overlap_t* h);
+/* KeyFrame::mPoints ([n,4], sensor frame) uploaded once, with the key frame's graph id.  *slot = 0, 1, 2, ... in call order. */
+lsd_status_t lsd_overlap_add_keyframe(lsd_overlap_t* h, const float* xyzi_host, int n, int32_t id, int32_t* slot);
+/* OverlapDetector::detect(keyframes, new_keyframes) (:63-110).  poses16 = mOdom of EVERY slot ([n_slots,16], double,
+ * row-major); keyframes = the loaded map's slots in mKeyFrames order (its first entry is what keyframe_id_map's default
+ * 0 points at, :189); new_keyframes = the fragment's slots; edges = graph_get_edges as [n_e][2] (prev id, next id).
+ * Writes up to cap overlaps in new key frame order; *n_found = overlaps found (may exceed cap). */
+lsd_status_t lsd_overlap_detect(lsd_overlap_t* h, const double* poses16, const int32_t* keyframes, int n_kf,
+                                const int32_t* new_keyframes, int n_new, const int32_t* edges, int n_e, lsd_overlap_result_t* out,
+                                int cap, int* n_found);
+/* Per new key frame of the last lsd_overlap_detect, in order.  out may be NULL. */
+lsd_status_t lsd_overlap_last_reports(lsd_overlap_t* h, lsd_overlap_report_t* out, int cap, int* n);
+/* Work of the last lsd_overlap_detect: kernel launches, and host round trips of the NDT stage (batched cost rounds).
+ * *target_buffers: sets of target tables the handle owns (the most one call needed); *targets_held: those a slot holds
+ * now (0 after lsd_overlap_detect).  Any output may be NULL. */
+lsd_status_t lsd_overlap_last_stats(lsd_overlap_t* h, long long* launches, int* rounds, int* target_buffers, int* targets_held);
+/* Hands back the tables the parity taps (lsd_overlap_fitness, lsd_overlap_match) built and kept; lsd_overlap_detect does
+ * this itself when it returns. */
+lsd_status_t lsd_overlap_release_targets(lsd_overlap_t* h);
+/* find_candidates (:113-145), pure host (works without a device).  poses16 / ids = mOdom / mId of slots 0 .. n_slots - 1;
+ * new_slot and every entry of keyframes must lie in that range (LSD_ERR_INVALID otherwise).  The 10-NN over the key
+ * frames' translations uses float points and float squared distances ((dx dx + dy dy) + dz dz); equal distances keep the
+ * order of `keyframes`.  get_connection_count is the reference's level-counted search (visited marked on pop).
+ * *n_cand = candidates (slots, in 10-NN order; may exceed cap). */
+lsd_status_t lsd_overlap_find_candidates(const lsd_overlap_params_t* p, const double* poses16, const int32_t* ids, int n_slots,
+                                         const int32_t* keyframes, int n_kf, const int32_t* edges, int n_e, int32_t new_slot,
+                                         int32_t* cand_out, int cap, int* n_cand);
+/* (new->mOdom.inverse() * cand->mOdom).matrix().cast<float>() (:159): Isometry3d inverse and product in double, each
+ * sum left to right, rounded to float.  Pure host. */
+void lsd_overlap_guess(const double* T_new16, const double* T_cand16, float* guess16);
+/* Eigen::Isometry3f(ndt_final).inverse().matrix() (:198), in float.  Pure host. */
+void lsd_overlap_finetune_guess(const float* ndt_final16, float* guess16);
+/* Parity tap: calc_fitness_score(target, source, T, max_range) (:225-263) through the batched kernel.  The target is
+ * filtered in its own frame; the source is transformed by T in float (PCL's order, no fused multiply-add) and filtered;
+ * each kept source point takes its exact nearest neighbour in the filtered target and counts when d2 <= max_range.
+ * score = sum d2 / counted (DBL_MAX when none), inlier_ratio = counted / kept (0 when none).  *target_incomplete: the
+ * filtered target's point map refused points, so every search scanned the whole filtered target.  Outputs may be NULL. */
+lsd_status_t lsd_overlap_fitness(lsd_overlap_t* h, int32_t target_slot, int32_t source_slot, const float* T16, double max_range,
+                                 double* score, double* inlier_ratio, int* n_counted, int* n_filtered, int* target_incomplete);
+/* Parity tap: the coarse stage alone for an explicit pair list (new_slots[i] is the NDT target, cand_slots[i] the source,
+ * guesses16 double [n,16]); the pairs may span several targets.  serial = 0: batched as in lsd_overlap_detect; serial = 1:
+ * the same pairs one after another through the single-pair kernels of lsd_reg on this handle's tables (the bit-exactness
+ * reference: a separate lsd_reg handle builds its own NDT table, whose double atomic sums may differ in the last bits
+ * from build to build).  Per pair: final NDT pose (double [n,16]),
+ * converged, iterations, getFitnessScore(fitness_score_max_range) at that pose (DBL_MAX when not converged).  Any output
+ * may be NULL.  *launches / *rounds: kernel launches and host round trips (batched cost evaluations) of the call. */
+lsd_status_t lsd_overlap_match(lsd_overlap_t* h, const int32_t* new_slots, const int32_t* cand_slots, const double* guesses16, int n,
+                               int serial, double* final16, int32_t* converged, int32_t* iterations, double* fitness, long long* launches, int* rounds);
+/* The LM iteration log of pair i of the last lsd_overlap_match / detect, same layout as lsd_reg_iteration_log. */
+lsd_status_t lsd_overlap_iteration_log(lsd_overlap_t* h, int i, double* out4_per_iter, int cap_iters, int* n_iters);
+
+/* ------------------------------------------------------------------------------------------
  * Detection voxelizer (config 5) — replaces sensor_driver/inference/voxelize:
  * Preprocess::forward (preprocess_kernel.cu:56-101: sliding window of max_frame_num frames, older frames
  * re-projected by a 3x4 motion, time channel + 0.1) and Voxelization::forward (voxelization_kernel.cu:

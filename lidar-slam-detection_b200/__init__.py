@@ -12,6 +12,8 @@ from .capi import (  # noqa: F401
     state_boxminus, state_boxplus, ImuProcess, eskf_predict, IMU_INITIALIZING, keyframe_filter, LocalMap, LOCALMAP_NONE, keyframe_save, keyframe_load, ERR_IO, ScanContext, FastLio,
     LoopDetector, find_loop_candidates, loop_information_matrix, LOOP_SKIPPED, LOOP_NO_CANDIDATES, LOOP_COARSE_REJECT,
     LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND, GlobalAligner, galign_merge_candidates,
+    OverlapDetector, overlap_find_candidates, overlap_guess, overlap_finetune_guess, OVERLAP_NO_CANDIDATES, OVERLAP_NO_MATCH,
+    OVERLAP_GICP_DIVERGED, OVERLAP_GICP_REJECT, OVERLAP_FOUND,
     FloorDetector, ransac_replay, FLOOR_MAPPING, FLOOR_GROUND, FLOOR_RENDER, FLOOR_FOUND, FLOOR_EMPTY, FLOOR_FEW_CANDIDATES,
     FLOOR_NO_MODEL, FLOOR_FEW_INLIERS, FLOOR_NOT_VERTICAL)
 from . import capi  # noqa: F401

@@ -85,6 +85,28 @@ class GalignMatch(C.Structure):
                 ("converged", C.c_int32), ("iterations", C.c_int32), ("score", C.c_double), ("accepted", C.c_int32)]
 
 
+class OverlapParams(C.Structure):
+    _fields_ = [("distance_thresh", C.c_double), ("candidate_link_dist", C.c_int32), ("max_candidate_num", C.c_int32),
+                ("fitness_score_max_range", C.c_double), ("fitness_score_thresh", C.c_double),
+                ("fitness_inlier_thresh", C.c_double), ("inlier_max_range", C.c_double), ("filter_range", C.c_double),
+                ("filter_min_z", C.c_float), ("coarse", RegParams), ("accurate", RegParams)]
+
+
+class OverlapResult(C.Structure):
+    _fields_ = [("key1", C.c_int32), ("key2", C.c_int32), ("relpose16", C.c_double * 16), ("score", C.c_double),
+                ("coarse_score", C.c_double)]
+
+
+class OverlapReport(C.Structure):
+    _fields_ = [("new_slot", C.c_int32), ("decision", C.c_int32), ("n_candidates", C.c_int32), ("n_prescreened", C.c_int32),
+                ("best_slot", C.c_int32), ("n_accum", C.c_int32), ("accum_incomplete", C.c_int32), ("best_score", C.c_double),
+                ("score", C.c_double)]
+
+
+# what OverlapDetector.detect decided for each new key frame (LSD_OVERLAP_*)
+OVERLAP_NO_CANDIDATES, OVERLAP_NO_MATCH, OVERLAP_GICP_DIVERGED, OVERLAP_GICP_REJECT, OVERLAP_FOUND = range(5)
+
+
 # what LoopDetector.detect decided for each new key frame (LSD_LOOP_*)
 LOOP_SKIPPED, LOOP_NO_CANDIDATES, LOOP_COARSE_REJECT, LOOP_GICP_DIVERGED, LOOP_GICP_REJECT, LOOP_FOUND = range(6)
 
@@ -228,6 +250,20 @@ SIGNATURES = [
     ("lsd_galign_match", _i, [_vp, C.c_int32, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, C.POINTER(C.c_longlong), _pi]),
     ("lsd_galign_iteration_log", _i, [_vp, _i, _vp, _i, _pi]),
     ("lsd_galign_cost", _i, [_vp, C.c_int32, C.c_int32, _vp, _i, _vp, _vp, C.POINTER(_d), _pi]),
+    ("lsd_overlap_default_params", None, [C.POINTER(OverlapParams)]),
+    ("lsd_overlap_create", _i, [_pp, C.POINTER(OverlapParams)]),
+    ("lsd_overlap_destroy", _i, [_vp]),
+    ("lsd_overlap_add_keyframe", _i, [_vp, _vp, _i, C.c_int32, C.POINTER(C.c_int32)]),
+    ("lsd_overlap_detect", _i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _pi]),
+    ("lsd_overlap_last_reports", _i, [_vp, _vp, _i, _pi]),
+    ("lsd_overlap_last_stats", _i, [_vp, C.POINTER(C.c_longlong), _pi, _pi, _pi]),
+    ("lsd_overlap_release_targets", _i, [_vp]),
+    ("lsd_overlap_find_candidates", _i, [C.POINTER(OverlapParams), _vp, _vp, _i, _vp, _i, _vp, _i, C.c_int32, _vp, _i, _pi]),
+    ("lsd_overlap_guess", None, [_vp, _vp, _vp]),
+    ("lsd_overlap_finetune_guess", None, [_vp, _vp]),
+    ("lsd_overlap_fitness", _i, [_vp, C.c_int32, C.c_int32, _vp, _d, C.POINTER(_d), C.POINTER(_d), _pi, _pi, _pi]),
+    ("lsd_overlap_match", _i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, C.POINTER(C.c_longlong), _pi]),
+    ("lsd_overlap_iteration_log", _i, [_vp, _i, _vp, _i, _pi]),
     ("lsd_vfe_default_params", None, [C.POINTER(VfeParams)]),
     ("lsd_vfe_create", _i, [_pp, C.POINTER(VfeParams)]),
     ("lsd_vfe_destroy", _i, [_vp]),
@@ -933,6 +969,145 @@ class GlobalAligner:
         check(lib.lsd_galign_cost(self.h, int(new_slot), int(ref_slot), _ptr(T), int(update), _ptr(H) if deriv else None,
                                   _ptr(b) if deriv else None, C.byref(e), C.byref(nc)))
         return e.value, H, b, nc.value
+
+
+def _overlap_params(**kw) -> OverlapParams:
+    p = OverlapParams()
+    lib.lsd_overlap_default_params(C.byref(p))
+    for k, v in kw.items():
+        if k in ("coarse", "accurate"):          # dict of lsd_reg_params_t fields
+            for kk, vv in v.items():
+                if not hasattr(p.coarse, kk):
+                    raise TypeError(f"unknown matcher parameter {kk}")
+                setattr(getattr(p, k), kk, vv)
+        elif hasattr(p, k):
+            setattr(p, k, v)
+        else:
+            raise TypeError(f"unknown overlap-detector parameter {k}")
+    return p
+
+
+def _edges(a) -> np.ndarray:
+    e = np.ascontiguousarray(a, np.int32).reshape(-1, 2) if len(a) else np.zeros((0, 2), np.int32)
+    return np.ascontiguousarray(e)
+
+
+class OverlapDetector:
+    """OverlapDetector (overlap_merge.hpp) of map merging on the device: key frames of both maps are added once with their
+    graph ids (clouds stay in device memory, addressed by slot); detect() finds the candidates of every new key frame of a
+    fragment, prescreens and NDT-aligns all (new, candidate) pairs in batches, refines each new key frame's best
+    candidate with GICP against the candidate accumulated with its graph neighbours and returns the overlaps."""
+
+    def __init__(self, **kw):
+        self.h = None
+        self.params = _overlap_params(**kw)
+        self.h = C.c_void_p()
+        check(lib.lsd_overlap_create(C.byref(self.h), C.byref(self.params)))
+        self.ids = []
+
+    def close(self):
+        if self.h:
+            lib.lsd_overlap_destroy(self.h)
+        self.h = None
+
+    __del__ = close
+
+    def add_keyframe(self, pts, kf_id: int) -> int:
+        pts = _f32(pts)
+        slot = C.c_int32()
+        check(lib.lsd_overlap_add_keyframe(self.h, _ptr(pts), pts.shape[0], int(kf_id), C.byref(slot)))
+        self.ids.append(int(kf_id))
+        return slot.value
+
+    def detect(self, poses, keyframes, new_keyframes, edges) -> list[dict]:
+        """poses: mOdom of every slot [n_slots, 4, 4]; keyframes: the loaded map's slots (mKeyFrames order); new_keyframes:
+        the fragment's slots; edges: graph edges as (prev id, next id) pairs.  One dict per overlap."""
+        P, kf, nk, E = _poses(poses), _slots(keyframes), _slots(new_keyframes), _edges(edges)
+        cap = max(nk.size, 1)
+        out = (OverlapResult * cap)()
+        n = C.c_int()
+        check(lib.lsd_overlap_detect(self.h, _ptr(P), _ptr(kf), kf.size, _ptr(nk), nk.size, _ptr(E), E.shape[0], out, cap, C.byref(n)))
+        return [dict(key1=r.key1, key2=r.key2, relpose=np.array(r.relpose16).reshape(4, 4), score=r.score,
+                     coarse_score=r.coarse_score) for r in out[:n.value]]
+
+    def reports(self) -> list[dict]:
+        """What the last detect() decided for each new key frame (decision: OVERLAP_*)."""
+        n = C.c_int()
+        check(lib.lsd_overlap_last_reports(self.h, None, 0, C.byref(n)))
+        out = (OverlapReport * max(n.value, 1))()
+        check(lib.lsd_overlap_last_reports(self.h, out, n.value, C.byref(n)))
+        return [{k: getattr(r, k) for k, _ in OverlapReport._fields_} for r in out[:n.value]]
+
+    def stats(self) -> dict:
+        """Work of the last detect(): kernel launches, host round trips of the NDT stage; target table sets owned / held."""
+        ln, rd, tb, th = C.c_longlong(), C.c_int(), C.c_int(), C.c_int()
+        check(lib.lsd_overlap_last_stats(self.h, C.byref(ln), C.byref(rd), C.byref(tb), C.byref(th)))
+        return dict(launches=ln.value, rounds=rd.value, target_buffers=tb.value, targets_held=th.value)
+
+    def release_targets(self):
+        """Hand back the tables fitness() and match() built and kept (detect() releases its own when it returns)."""
+        check(lib.lsd_overlap_release_targets(self.h))
+
+    def find_candidates(self, poses, keyframes, new_slot: int, edges) -> np.ndarray:
+        return overlap_find_candidates(poses, self.ids, keyframes, new_slot, edges, params=self.params)
+
+    def fitness(self, target_slot: int, source_slot: int, T, max_range: float) -> dict:
+        """calc_fitness_score(target, source, T, max_range) of the reference's merge (filtered clouds)."""
+        Tf = np.ascontiguousarray(T, np.float32)
+        sc, ratio = C.c_double(), C.c_double()
+        nr, nf, inc = C.c_int(), C.c_int(), C.c_int()
+        check(lib.lsd_overlap_fitness(self.h, int(target_slot), int(source_slot), _ptr(Tf), float(max_range), C.byref(sc), C.byref(ratio),
+                                      C.byref(nr), C.byref(nf), C.byref(inc)))
+        return dict(score=sc.value, inlier_ratio=ratio.value, n_counted=nr.value, n_filtered=nf.value, target_incomplete=bool(inc.value))
+
+    def match(self, new_slots, cand_slots, guesses, serial: bool = False) -> dict:
+        """The coarse stage alone for an explicit pair list, batched or (serial) one pair at a time through lsd_reg's
+        single-pair kernels on the same tables (parity tap and baseline)."""
+        ns, cs = _slots(new_slots), _slots(cand_slots)
+        n = cs.size
+        G = np.ascontiguousarray(guesses, np.float64).reshape(n, 4, 4)
+        T = np.zeros((n, 4, 4)); cv = np.zeros(n, np.int32); it = np.zeros(n, np.int32); fit = np.zeros(n)
+        ln, rd = C.c_longlong(), C.c_int()
+        check(lib.lsd_overlap_match(self.h, _ptr(ns), _ptr(cs), _ptr(G), n, int(bool(serial)), _ptr(T), _ptr(cv), _ptr(it), _ptr(fit), C.byref(ln), C.byref(rd)))
+        logs = []
+        for i in range(n):
+            m = C.c_int()
+            check(lib.lsd_overlap_iteration_log(self.h, i, None, 0, C.byref(m)))
+            lg = np.zeros((max(m.value, 1), 4))
+            check(lib.lsd_overlap_iteration_log(self.h, i, _ptr(lg), m.value, C.byref(m)))
+            logs.append(lg[:m.value])
+        return dict(final=T, converged=cv.astype(bool), iterations=it, fitness=fit, launches=ln.value, rounds=rd.value,
+                    iteration_logs=logs)
+
+
+def overlap_find_candidates(poses, ids, keyframes, new_slot: int, edges, params=None, **kw) -> np.ndarray:
+    """OverlapDetector::find_candidates (pure host, no device needed): candidate slots in 10-NN order."""
+    p = params if params is not None else _overlap_params(**kw)
+    P, kf, E = _poses(poses), _slots(keyframes), _edges(edges)
+    idv = np.ascontiguousarray(ids, np.int32)
+    if idv.size != P.shape[0]:
+        raise ValueError("one id and one pose per slot")
+    cand = np.zeros(max(kf.size, 1), np.int32)
+    n = C.c_int()
+    check(lib.lsd_overlap_find_candidates(C.byref(p), _ptr(P), _ptr(idv), P.shape[0], _ptr(kf), kf.size, _ptr(E), E.shape[0], int(new_slot),
+                                          _ptr(cand), cand.size, C.byref(n)))
+    return cand[:n.value].copy()
+
+
+def overlap_guess(T_new, T_cand) -> np.ndarray:
+    """(new.inverse() * cand).matrix().cast<float>() of the reference's prescreen and NDT guess (pure host)."""
+    a, b = np.ascontiguousarray(T_new, np.float64), np.ascontiguousarray(T_cand, np.float64)
+    out = np.zeros((4, 4), np.float32)
+    lib.lsd_overlap_guess(_ptr(a), _ptr(b), _ptr(out))
+    return out
+
+
+def overlap_finetune_guess(ndt_final) -> np.ndarray:
+    """Eigen::Isometry3f(ndt_final).inverse().matrix() in float (pure host)."""
+    a = np.ascontiguousarray(ndt_final, np.float32)
+    out = np.zeros((4, 4), np.float32)
+    lib.lsd_overlap_finetune_guess(_ptr(a), _ptr(out))
+    return out
 
 
 def galign_merge_candidates(cand_idx, cand_dist, cand_shift, n_cand, dist_thres: float = 0.30):
